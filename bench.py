@@ -1,15 +1,20 @@
 #!/usr/bin/env python
-"""bench.py -- LM iterations/sec on the batched SE3 pose graph of BASELINE.json, on N B200s.
+"""bench.py -- LM iterations/sec on the batched SE3 pose graph of BASELINE.json, on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     (N>1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...)
 
 HEADLINE (value / e2e / roofline / cpu_baseline / parity): BASELINE.json's scaling configuration C5 -- sphere-like SE3 pose graph,
-2 500 poses, 4 949 edges + 1 prior (m = 29 700, n = 15 000), GLOBAL batch 4096 sharded over the N ranks (strong scaling: N=1 holds all
-4096 problems, N=8 holds 512 each), LevenbergMarquardt(10 iterations, damping 1e-3, adaptive + ellipsoidal damping, tolerances 0)
+2 500 poses, 4 949 edges + 1 prior (m = 29 700, n = 15 000), GLOBAL batch 2048 sharded over the N ranks (strong scaling: N=1 holds all
+2048 problems, N=8 holds 256 each), LevenbergMarquardt(10 iterations, damping 1e-3, adaptive + ellipsoidal damping, tolerances 0)
 with the block-sparse multifrontal Cholesky (BaspachoSparseSolver, layout "front") on SparseLinearization, fp64.
 A "step" = one LM solve (10 iterations of linearize -> Gram -> damped factor -> substitutions -> retract -> error -> accept/reject) of
-the whole 4096-problem batch; value = LM iterations per second of that batch.
+the whole 2048-problem batch; value = LM iterations per second of that batch.  BASELINE.json spreads 4096 problems over 8 GPUs; 2048 is
+what one 80 GB H100 holds with room to spare: about 23 MB per problem (factor panels, Jacobian, Gram blocks, vectors) plus a 10 GB
+chunked update-matrix arena.
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step returned (see dump_outputs) as .npy files; inputs
+are seeded, so two builds run with the same arguments can be compared output for output.
 
 BESIDE it, never mixed into `value` (key `dense_c2`): BASELINE.json's single-GPU configuration C2 -- 256 poses, batch 256 per GPU
 (weak), LM + dense Cholesky -- with the dense DMMA factor's roofline and the GPU-library baseline (torch bmm + linalg.cholesky +
@@ -35,11 +40,11 @@ LM_ITERS = 10
 LM_KW = dict(damping=1e-3, adaptive_damping=True, ellipsoidal_damping=True)
 # ---- headline: C5 ----
 C5_RINGS, C5_PER_RING = 50, 50
-C5_GLOBAL_BATCH = int(os.environ.get("THB_BENCH_C5_BATCH", "4096"))
+C5_GLOBAL_BATCH = int(os.environ.get("THB_BENCH_C5_BATCH", "2048"))
 C5_LAYOUT = os.environ.get("THB_BENCH_C5_LAYOUT", "front")
-METRIC = "LM iterations/sec on batched SE3 pose-graph (2500 poses, global batch 4096 over N GPUs, LM + block-sparse Cholesky, fp64)"
-UNIT = "LM iterations/s of the 4096-problem batch (one iteration = one LM step of all 4096 pose graphs)"
-WORKLOAD = ("C5: sphere-like SE3 pose graph (50 rings x 50 = 2 500 poses, 4 949 edges + 1 prior; m=29 700, n=15 000), global batch 4096 "
+METRIC = f"LM iterations/sec on batched SE3 pose-graph (2500 poses, global batch {C5_GLOBAL_BATCH} over N GPUs, LM + block-sparse Cholesky, fp64)"
+UNIT = f"LM iterations/s of the {C5_GLOBAL_BATCH}-problem batch (one iteration = one LM step of all {C5_GLOBAL_BATCH} pose graphs)"
+WORKLOAD = (f"C5: sphere-like SE3 pose graph (50 rings x 50 = 2 500 poses, 4 949 edges + 1 prior; m=29 700, n=15 000), global batch {C5_GLOBAL_BATCH} "
             "sharded over the ranks, LM(10 it, damping 1e-3, adaptive+ellipsoidal) + BaspachoSparseSolver(layout=front: multifrontal "
             "block-sparse Cholesky) on SparseLinearization, fp64")
 # ---- beside it: C2 ----
@@ -49,24 +54,25 @@ C2_WORKLOAD = ("C2: synthetic SE3 pose-graph (pose_graph_cube shape: 256 poses, 
 CPU_SAMPLE_ITEMS = 32
 # sparse CPU arms: one process per batch item, as many items as the host has cores (bounded: 16..128) -- the reference's per-item loop on ALL cores
 C5_CPU_ITEMS = int(os.environ.get("THB_BENCH_CPU_ITEMS", str(max(16, min(os.cpu_count() or 16, 128)))))
+DUMP_ITEMS = 128   # --dump-outputs: final poses of this many batch items (31 MB in float64), chosen by a fixed seed
 
 
 def _measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0), "fallback"
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0), "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """Samples nvidia-smi clocks / throttle reasons / power limit during the timed region."""
 
     def __init__(self, index=0):
         self.rows, self.proc, self.index = [], None, index
 
     def start(self):
         q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
-             "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-lms", "100", "-i", str(self.index)],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
@@ -88,18 +94,19 @@ class ClockSampler:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, plim, reasons = [], [], [], set()
         for r in self.rows:
             try:
                 sm.append(float(r[1]))
                 mx.append(float(r[2]))
+                plim.append(float(r[9]))
             except Exception:
                 continue
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[5:9]):
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return dict(sm_mhz=float(np.median(sm)) if sm else None, sm_max_mhz=max(mx) if mx else None, reasons=sorted(reasons),
-                    samples=len(sm))
+                    power_limit_w=max(plim) if plim else None, samples=len(sm))
 
 
 def _host_threads():
@@ -146,9 +153,9 @@ def make_c5_data(batch, seed, device="cpu"):
 
 # ------------------------------------------------------------------------------------------------ --impl reference
 def run_reference(args):
-    """--impl reference: the reference's own CPU algorithm for the headline workload (oracle port; /root/reference is Python and does
-    not travel to the GPU box), all host cores, rank 0 only.  Each step = the LM solve of a bounded sample (C5_CPU_ITEMS of the 4096
-    items); value = LM iterations/s of the 4096-batch assuming the reference's per-item loop scales linearly in the batch."""
+    """--impl reference: the reference's own CPU algorithm for the headline workload (numpy port in oracle/), all host cores, rank 0
+    only.  Each step = the LM solve of a bounded sample (C5_CPU_ITEMS of the batch items); value = LM iterations/s of the whole batch
+    assuming the reference's per-item loop scales linearly in the batch."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -171,7 +178,7 @@ def run_reference(args):
                 config=dict(workload=WORKLOAD, global_batch=C5_GLOBAL_BATCH,
                             note="CPU oracle port of the reference path (SparseLinearization + one sparse direct factorisation per item, SuperLU "
                                  f"standing in for CHOLMOD/BaSpaCho-CPU); {sample}-item sample timed ({t_sample:.2f} s per LM solve), scaled linearly "
-                                 "to the 4096-item batch"),
+                                 f"to the {C5_GLOBAL_BATCH}-item batch"),
                 cpu_baseline=dict(value=value, unit=UNIT, cores=used, host_cores=cores, kind="port",
                                   sample=f"{sample} of {C5_GLOBAL_BATCH} batch items x {LM_ITERS} LM iterations per step, {len(times)} steps"),
                 e2e=dict(value=value, unit=UNIT, h2d_bytes_per_step=0, d2h_bytes_per_step=0), gpu_launches=0)
@@ -187,6 +194,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-c2", action="store_true", help="skip the dense C2 leg reported beside the headline")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -265,6 +273,8 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     value = LM_ITERS * 1e3 / ms_step
     final_err = out["info"].last_err.clone()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out["values"], out["info"], names_pose)
 
     # ---- e2e: pinned host inputs -> device, public API, solution + error back to pinned host memory, every step ----
     host_poses, host_meas = data["poses"].pin_memory(), data["meas"].pin_memory()
@@ -306,7 +316,7 @@ def main():
     stats = {k: (float(v) if not isinstance(v, str) else v) for k, v in dict(solver.symbolic_stats).items()}
     flops_item = float(stats.get("flops", 0.0))
     nnz_l = float(stats.get("nnz_L", 0.0))
-    # fp64 peak: MEASURED_PEAKS.json has no fp64 entry -> cuBLAS dgemm 8192^3 measured live, same method as the driver's bf16 peak
+    # fp64 peak: MEASURED_PEAKS.json has no fp64 entry -> cuBLAS dgemm 8192^3 measured live
     am = torch.randn(8192, 8192, dtype=torch.float64, device=device)
     bm = torch.randn(8192, 8192, dtype=torch.float64, device=device)
     torch.matmul(am, bm)
@@ -321,14 +331,14 @@ def main():
     peak_tf = 2 * 8192 ** 3 / (best * 1e-3) / 1e12
     del am, bm
     peaks, peaks_src = _measured_peaks()
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
     # algorithmic bytes of one numeric factorisation per item: AtA blocks read + L written (DESIGN.md 4); the substitutions read L twice
     ata_doubles = float(sum(int(a) * int(bb) for a, bb in zip(solver._gram_arrays["blk_rows"], solver._gram_arrays["blk_cols"])))
     bytes_factor = 8.0 * (ata_doubles + nnz_l) * B
     t_flops, t_bytes = flops_item * B / (peak_tf * 1e12), bytes_factor / (hbm * 1e9)
     achieved_tf = flops_item * B / (ms_numeric * 1e-3) / 1e12
     roofline = dict(bound="tensor", kernel=f"thb_front_factor_f64 + Gram: one numeric factorisation of {B} items (multifrontal: shared-memory front kernel "
-                    "+ DMMA dense kernel in partial mode; kernel list: profiles/r02_*_launch_agg.txt)",
+                    "+ DMMA dense kernel in partial mode)",
                     achieved=achieved_tf, peak=peak_tf, unit="TFLOP/s", frac=achieved_tf / peak_tf,
                     traffic=None, flops_per_item=flops_item, nnz_L=nnz_l, algorithmic_bytes=bytes_factor, ms_per_factorisation=ms_numeric,
                     hbm_frac_of_algorithmic_bytes=bytes_factor / (ms_numeric * 1e-3) / (hbm * 1e9),
@@ -336,15 +346,7 @@ def main():
                     substitutions=dict(ms=ms_subst, algorithmic_bytes=16.0 * nnz_l * B, hbm_frac=16.0 * nnz_l * B / (ms_subst * 1e-3) / (hbm * 1e9)),
                     peak_source="fp64 cuBLAS dgemm 8192^3 measured live in this run (MEASURED_PEAKS.json carries no fp64 figure; "
                                 f"its bf16/HBM entries [{peaks_src}]: {peaks.get('bf16_tflops')} TF/s, {hbm} GB/s)",
-                    share_of_step=ms_numeric * LM_ITERS / ms_step,
-                    # the largest single kernel of the factorisation, from the committed captures (NOT measured in this run): its traffic
-                    # is the per-kernel dram figure the contract's `traffic` key asks for; the call above is ~100 launches of 6 kernels
-                    dominant_kernel=dict(name="front_small_kernel<1024>", share_of_linear_solve=0.283,
-                                         share_source="profiles/r02m_c5_B512_front_launch_agg.txt (ncu --metrics gpu__time_duration.sum, one solve, B=512)",
-                                         ncu_launch="depth-6 launch of C5, B=512: 6 fronts (w 36-66, b 192-372) x 512 items, 26.3 MFLOP per item",
-                                         duration_ms=1.47, achieved_tflops=9.2, dmma_pipe_pct=29.5, traffic=2.92e9,
-                                         algorithmic_bytes=2.40e9, traffic_over_algorithmic=1.22,
-                                         ncu_source="profiles/r02l_front_small_1024_ncu_full_details.txt, r02l_front_kernels_ncu_summary.txt"))
+                    share_of_step=ms_numeric * LM_ITERS / ms_step)
 
     # ---- bench-size parity: first-iteration delta and final error of the first items vs the CPU oracle's run on the same items.
     # Every rank runs the extra (untimed) solve so that the per-iteration collectives stay matched; rank 0 compares. ----
@@ -374,6 +376,22 @@ def main():
                               "SparseLinearization + per-item sparse direct factorisation (SuperLU standing in for CHOLMOD / BaSpaCho-CPU)",
                        final_err_mean_sample=float(e_ref.mean()))
 
+    config = dict(workload=WORKLOAD, global_batch=C5_GLOBAL_BATCH, batch_per_gpu=B, num_poses=len(poses), num_edges=len(data["edges"]),
+                  rows=int(lin.num_rows), cols=int(lin.num_cols), lm_iterations_per_step=LM_ITERS, problem_iterations_per_s=value * C5_GLOBAL_BATCH,
+                  layout=solver.effective_layout, symbolic=stats,
+                  l2="working set per iteration (factor panels + update-matrix arena, > 10 GB per rank) >> 50 MB L2, no flush needed",
+                  parallelism=f"batch sharded over {world} GPU(s); per LM iteration one all-reduce of the reject / item counts (+ one of the "
+                              "solve-failure flag), NCCL",
+                  cuda_graph=bool(opt.cuda_graph), gpu=torch.cuda.get_device_name(device),
+                  peak_memory_gb=torch.cuda.max_memory_allocated(device) / 1e9)
+    # The C5 buffers (about 55 GB at batch 2048) are released before the C2 leg: with its dense A and the library baseline's dense
+    # copies the C2 leg needs about 40 GB more, and both together do not fit an 80 GB device.
+    del layer, opt, objective, poses, data, dev_inputs, out, lin, solver, A64, b64, Atb, step_resident, step_e2e, cb
+    del host_poses, host_meas, dev_pose_buf, dev_meas_buf, host_out, host_err
+    import gc
+    gc.collect()
+    torch.cuda.empty_cache()
+
     # ================================================= beside it: C2 dense =================================================
     c2 = None
     if not args.no_c2:
@@ -391,14 +409,7 @@ def main():
     line = dict(
         metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=warmup, ms_per_step=ms_step, higher_is_better=True,
         scaling="strong", vs_baseline=None, dtype="f64", data="synthetic",
-        config=dict(workload=WORKLOAD, global_batch=C5_GLOBAL_BATCH, batch_per_gpu=B, num_poses=len(poses), num_edges=len(data["edges"]),
-                    rows=int(lin.num_rows), cols=int(lin.num_cols), lm_iterations_per_step=LM_ITERS, problem_iterations_per_s=value * C5_GLOBAL_BATCH,
-                    layout=solver.effective_layout, symbolic=stats,
-                    l2="working set per iteration (factor panels + update-matrix arena, > 10 GB per rank) >> 126 MB L2, no flush needed",
-                    parallelism=f"batch sharded over {world} GPU(s); per LM iteration one all-reduce of the reject / item counts (+ one of the "
-                                "solve-failure flag), NCCL",
-                    cuda_graph=bool(opt.cuda_graph)),
-        clocks=clocks,
+        config=config, clocks=clocks,
         e2e=dict(value=LM_ITERS * 1e3 / ms_e2e, unit=UNIT, ms_per_step=ms_e2e, steps=e2e_steps, h2d_bytes_per_step=h2d, d2h_bytes_per_step=d2h),
         gpu_launches=launches, roofline=roofline,
         phases_ms_per_iteration=dict(linearize=ms_lin, linear_solve=ms_solve, numeric_factorisation=ms_numeric, substitutions=ms_subst),
@@ -409,6 +420,18 @@ def main():
         sys.exit(3)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(dirname, values, info, names_pose):
+    """What the timed LM solve returned in its last step, float64: `poses.npy` [DUMP_ITEMS, poses, 3, 4] = the optimised poses of a fixed
+    sample of batch items (torch.randperm with seed 0, ascending), `last_err.npy` [B] = the final error of every batch item."""
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    B = info.last_err.shape[0]
+    items = torch.randperm(B, generator=torch.Generator().manual_seed(0))[:min(DUMP_ITEMS, B)].sort().values.to(info.last_err.device)
+    poses = torch.stack([values[n][items] for n in names_pose], 1)
+    np.save(os.path.join(dirname, "poses.npy"), poses.double().cpu().numpy())
+    np.save(os.path.join(dirname, "last_err.npy"), info.last_err.double().cpu().numpy())
 
 
 def dense_c2_leg(th, lib, _lib, device, rank, world, pg, timed, peak_tf, steps, with_cpu):
@@ -451,8 +474,7 @@ def dense_c2_leg(th, lib, _lib, device, rank, world, pg, timed, peak_tf, steps, 
                unit="LM iterations/s (one iteration = one LM step of a 256-problem batch; summed over the GPUs: weak scaling)",
                ms_per_step=ms_step, steps=steps, batch_per_gpu=C2_BATCH, cols=int(n), final_err_mean=float(out["info"].last_err.mean().item()),
                roofline=dict(bound="tensor", kernel="chol_col_kernel (fp64 DMMA left-looking Cholesky, one launch = one batched factorisation of 256 matrices)",
-                             achieved=achieved_tf, peak=peak_tf, unit="TFLOP/s", frac=achieved_tf / peak_tf, traffic=34.40e9,
-                             traffic_note="dram bytes per launch from the round-1 ncu --set full capture (profiles/r01g_chol_col_ncu_full_details.txt)",
+                             achieved=achieved_tf, peak=peak_tf, unit="TFLOP/s", frac=achieved_tf / peak_tf, traffic=None,
                              algorithmic_bytes=8.0 * B * n * n, ms_per_factorisation=ms_factor, share_of_step=ms_factor * LM_ITERS / ms_step))
     # ---- GPU-library baseline: what the reference's dense path executes on this GPU for one linear solve of the same system ----
     if rank == 0:

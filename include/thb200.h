@@ -1,4 +1,4 @@
-/* libthb200 -- C ABI of the B200-native Theseus NLS hot path (linearize -> solve -> retract).
+/* libthb200 -- C ABI of the H100-native Theseus NLS hot path (linearize -> solve -> retract).
  *
  * This header is the drop-in boundary: plain C, device pointers + sizes + a cudaStream_t, no torch
  * types.  It replaces the pybind11 torch-extension modules of the reference's theseus/extlib and the
@@ -410,7 +410,7 @@ int thb_lm_control_f32(const float* delta, const float* Atb, const float* diag, 
  * Dense batched Gram for GENUINELY dense Jacobians (AutoDiffCostFunction with dim >> dof):  AtA [B,n,n] = A^T A,  A [B,m,n] row-major.
  * Replaces `At.bmm(A)` of theseus/optimizer/dense_linearization.py:58-62 where the block-sparse Gram (thb_gram_f64) has nothing to skip.
  * TMA-staged tiles (one 3-D tensor map over [B,m,n], cp.async.bulk.tensor + mbarrier ring) feeding the FP64 tensor pipe (mma.sync DMMA;
- * tcgen05 has no fp64 kind); the full symmetric matrix is written.  n must be even and A 16-byte aligned (else THB_ERR_UNSUPPORTED:
+ * wgmma has no fp64 kind); the full symmetric matrix is written.  n must be even and A 16-byte aligned (else THB_ERR_UNSUPPORTED:
  * the Python host then stays on thb_gram_f64).
  * ---------------------------------------------------------------------------------------------- */
 int thb_gram_dense_f64(const double* A, double* AtA, int64_t B, int64_t m, int64_t n, thb_stream_t stream);

@@ -7,7 +7,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100 with -m gpu)")
     if os.environ.get("THB_SIMT_EMULATION") == "1":
         # opt-in DRY RUN of the GPU tests on the host emulation of the kernels (tests/simt/emulation_mode.py); never set by the driver
         import importlib.util

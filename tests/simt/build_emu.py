@@ -87,7 +87,7 @@ def build(force: bool = False) -> str:
         return lib
     for f, g in gens.items():
         open(g, "w").write(texts[f])
-    cmd = ["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-DTHB_SIMT_EMU", "-DTHB_ARCH=100", "-Wno-unknown-pragmas",
+    cmd = ["g++", "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-DTHB_SIMT_EMU", "-DTHB_ARCH=90", "-Wno-unknown-pragmas",
            # the CUDA library exports host stubs with the SAME mangled kernel names: bind this library's references to its own definitions
            "-Wl,-Bsymbolic", "-fno-semantic-interposition", "-I", HERE, "-I", OUT_DIR] + [gens[f] for f in SOURCES] + ["-o", lib]
     r = subprocess.run(cmd, capture_output=True, text=True)

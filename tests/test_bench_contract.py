@@ -1,6 +1,6 @@
 """bench.py's output contract, checked without a GPU: (1) the `--impl reference` arm (CPU oracle port, the one arm that runs here)
 prints ONE JSON line with the keys the driver parses; (2) the device arm refuses to run without CUDA (there is no CPU fallback to time
-by accident); (3) the committed line of the final single-GPU run carries every key of the contract."""
+by accident); (3) the committed line of a single-H100 run carries every key of the contract."""
 import json
 import os
 import subprocess
@@ -26,7 +26,7 @@ def test_reference_arm_prints_one_contract_line():
     assert d["impl"] == "reference" and all(k in d for k in BASE_KEYS)
     assert d["value"] > 0 and d["higher_is_better"] is True and d["scaling"] == "strong" and d["dtype"] == "f64"
     assert d["e2e"]["value"] == d["value"] and d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
-    assert d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["cores"] == 2 and "2 of 4096" in d["cpu_baseline"]["sample"]
+    assert d["cpu_baseline"]["kind"] == "port" and d["cpu_baseline"]["cores"] == 2 and "2 of 2048" in d["cpu_baseline"]["sample"]
     assert "workload" in d["config"] and "model" not in d["config"]
 
 
@@ -42,7 +42,7 @@ def test_device_arm_does_not_run_without_cuda():
 
 
 def test_committed_final_line_has_every_contract_key():
-    d = json.loads(open(os.path.join(ROOT, "profiles", "r02n_bench_n1_line_final.json")).read())
+    d = json.loads(open(os.path.join(ROOT, "profiles", "h100_bench_n1_line.json")).read())
     for k in BASE_KEYS + ("clocks", "gpu_launches", "roofline"):
         assert k in d, k
     assert d["n_gpus"] == 1 and d["gpu_launches"] > 0 and d["vs_baseline"] is None

@@ -1,8 +1,7 @@
 """SURVEY.md 8(e) on hardware: the batch sharded over 2 GPUs (one process per GPU, NCCL) against the single-GPU run, per batch item.
 No kernel mixes batch items and no data-path collective exists; the only batch-global decisions (all items rejected -> retry, the
 linear-solve failure flag) are all-reduced, so every per-item quantity must be BITWISE the single-process one -- dense and sparse.
-Needs >= 2 GPUs (skipped on the one-GPU box; run with `gpurun --gpus 2 -- python -m pytest tests/test_gpu_nccl_sharded.py -m gpu`,
-log under profiles/)."""
+Needs >= 2 GPUs (skipped on a machine with one)."""
 import os
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""theseus_b200 -- a B200-native (sm_100a) implementation of the batched nonlinear-least-squares inner loop of
+"""theseus_b200 -- an H100-native (sm_90a) implementation of the batched nonlinear-least-squares inner loop of
 facebookresearch/theseus (linearize -> solve -> retract), behind the reference's own plugin API.
 
     import theseus_b200 as th

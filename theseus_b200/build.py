@@ -1,4 +1,4 @@
-"""Build libthb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libthb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m theseus_b200.build [--force]
 
@@ -18,8 +18,8 @@ LIBNAME = "libthb200.so"
 SOURCES = ["thb_costs.cu", "thb_gram.cu", "thb_chol_dense.cu", "thb_sparse.cu", "thb_sparse_lane.cu", "thb_symbolic.cu", "thb_lie_ops.cu", "thb_front.cu", "thb_gram_dense.cu"]
 HEADERS = ["thb_common.cuh", "thb_lie.cuh", os.path.join("..", "..", "include", "thb200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
-    "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-DTHB_ARCH=100",
+    "-gencode", "arch=compute_90a,code=sm_90a",
+    "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-DTHB_ARCH=90",
 ]
 
 
@@ -70,7 +70,7 @@ def build(force=False, verbose=True):
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
         if verbose and out.strip():
             print(out)
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", lib_path()] + objs + ["-lcudart"]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", lib_path()] + objs + ["-lcudart"]
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.check_call(cmd)

@@ -1,4 +1,4 @@
-// Batched dense Cholesky factor + solve with fused LM damping, fp64, for sm_100a.
+// Batched dense Cholesky factor + solve with fused LM damping, fp64, for sm_90a.
 //
 // Replaces torch.linalg.cholesky + torch.cholesky_solve + DenseSolver._apply_damping
 // (theseus/optimizer/linear/dense_solver.py:38-64,159-161).
@@ -20,8 +20,7 @@
 // written once and AtA read once (algorithmic bytes) instead of the read-modify-write sweeps of a right-looking update.
 // Solve: x = M^-1 rhs with the stored W_j (triangular solves become mat-vecs), one CTA per matrix, HBM-bound.
 //
-// FP64 has no tcgen05 kind; the FP64 tensor pipe of sm_100a is reached with mma.sync DMMA (measured on this pool:
-// 37.1 TFLOP/s DMMA vs 34.2 DFMA vs 35.4 cuBLAS dgemm, profiles/r01_ubench_fp64.txt).
+// wgmma has no fp64 kind; the FP64 tensor pipe of sm_90a is reached with mma.sync DMMA (m8n8k4).
 #include "thb_common.cuh"
 
 namespace thb {
@@ -153,8 +152,8 @@ __device__ __noinline__ int warp_potrf_inv(double* __restrict__ T, double* __res
 // block, zeros above the diagonal).  N == THB_CHOL_LEAF: one warp does it in registers.  Otherwise the same 2x2 recursion as one
 // level up: factor+invert T00, L10 = T10 W00^T, T11 -= L10 L10^T, factor+invert T11, W10 = -W11 L10 W00 -- the products as DMMA on
 // 8x8 tiles (one warp per tile).  Small leaves matter because the serial pivots are scalar FP64 instructions that compete for the
-// FP64 pipe with the DMMA stream of the co-resident CTA: a 32x32 register leaf costs 33-57 us there, four 8x8 leaves + tile
-// products a fraction of it (profiles/r01_chol_history.md).  The return value is valid on warp 0.
+// FP64 pipe with the DMMA stream of the co-resident CTA: four 8x8 leaves + tile products cost a fraction of one 32x32 register
+// leaf.  The return value is valid on warp 0.
 template <int N>
 __device__ __forceinline__ int block_factor_invert(double* __restrict__ T, double* __restrict__ Wb, int warp, int lane) {
   if constexpr (N <= THB_CHOL_LEAF) {

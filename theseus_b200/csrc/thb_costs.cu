@@ -635,8 +635,8 @@ __global__ void commit_kernel(VarDev<T> v, int64_t B, const uint8_t* __restrict_
 
 // ------------------------------------------------------------------------------------------------
 // LM control: one CTA per batch item reduces den over n columns (levenberg_marquardt.py:172-201); partial sums per thread, per warp
-// (shuffles) and per CTA (warp order) -- a fixed order, so the accept decision is reproducible.  (One WARP per item left 512 warps to
-// stream 3 x 61 MB at C5 B=512: 0.28 ms.)
+// (shuffles) and per CTA (warp order) -- a fixed order, so the accept decision is reproducible.  (One WARP per item leaves too few
+// warps to stream the three n-vectors of a large batch.)
 constexpr int kLmCtrlThreads = 256;
 template <typename T>
 __global__ void __launch_bounds__(kLmCtrlThreads) lm_control_kernel(const T* __restrict__ delta, const T* __restrict__ Atb, const T* __restrict__ diag, int64_t B,

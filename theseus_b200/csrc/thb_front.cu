@@ -1,4 +1,4 @@
-// Multifrontal (supernodal) batched block-sparse Cholesky, fp64, sm_100a -- numeric phase of layout "front".
+// Multifrontal (supernodal) batched block-sparse Cholesky, fp64, sm_90a -- numeric phase of layout "front".
 //
 // Replaces BaSpaCho's batched factor / solve behind NumericDecomposition::factor / solve
 // (theseus/extlib/baspacho_solver_cuda.cu:203-214, 282-287) for B problems that share ONE structure.  Symbolic side:
@@ -27,8 +27,8 @@ namespace thb {
 // its CTAs run their prologue (plan descriptors, inverse maps, zero fill -- nothing the predecessor writes) and then wait for the
 // predecessor's completion (griddepcontrol.wait, which also orders its memory) before the first dependent read or any global write.
 // ~300 launches per linear solve of 10-200 us each: the launch gap, the tail of the last wave and the prologue are what this was meant to
-// hide.  MEASURED (C5, B = 512): numeric phase unchanged, substitutions 7.6 -> 11.4 ms (early CTAs sit on the SMs' thread slots while
-// they wait) -- so the attribute is only set with THB_FRONT_PDL=1; without it the two instructions are no-ops.
+// hide.  It made the substitutions slower (early CTAs sit on the SMs' thread slots while they wait), so the attribute is only set
+// with THB_FRONT_PDL=1; without it the two instructions are no-ops.
 #ifdef THB_SIMT_EMU
 #define THB_PDL_TRIGGER() do { } while (0)
 #define THB_PDL_WAIT() do { } while (0)
@@ -38,7 +38,7 @@ namespace thb {
 #define THB_PDL_WAIT() asm volatile("griddepcontrol.wait;" ::: "memory")
 #define FRONT_LAUNCH(K, grid, block, smem, cs, arg) thb::front_launch_pdl(K, grid, block, smem, cs, arg)
 static inline bool front_pdl_enabled() {
-  static const bool on = [] { const char* e = getenv("THB_FRONT_PDL"); return e != nullptr && e[0] == '1'; }();   // opt-in: measured SLOWER at C5 B=512 (substitutions 7.6 -> 11.4 ms)
+  static const bool on = [] { const char* e = getenv("THB_FRONT_PDL"); return e != nullptr && e[0] == '1'; }();   // opt-in: slower substitutions (see above)
   return on;
 }
 template <typename A>
@@ -111,7 +111,7 @@ __device__ __forceinline__ double front_panel_in(const FrontArgs& a, const doubl
 //      written once from registers.
 constexpr int FRONT_WD_LD = 20;
 #ifndef FRONT_PL
-#define FRONT_PL 4   // panel elements a thread gathers per pass (their global loads are in flight together; 8 measured 2 % slower)
+#define FRONT_PL 4   // panel elements a thread gathers per pass (their global loads are in flight together)
 #endif
 constexpr int FRONT_MAX_CHILDREN = 8;   // fronts with more children are assembled by the scatter kernel of the dense path (frontal.py)
 
@@ -268,7 +268,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
   THB_PDL_WAIT();   // everything above reads the plan only; below: the children's update matrices, AtA, and every global write
 #ifndef THB_SIMT_EMU
   // the children's update matrices (lower triangles) are read element by element by the gathers below: ask L2 for their lines now, so that
-  // the gathers find them on chip (fire and forget: no register, no stall; the ncu source view showed 45 % of all stall samples on those loads)
+  // the gathers find them on chip (fire and forget: no register, no stall)
   for (int q = 0; a.prefetch != 0 && q < nch; q++) {
     const int64_t* PC = p.pc + (int64_t)(c_begin + q) * 6;
     const double* csrc = a.arena_child + item * p.arena_size + PC[0];
@@ -322,7 +322,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
   // ---- blocked left-looking factorisation of the panel, 8 columns at a time ----
   const int nbk = w8 / 8, nrt = (w8 + b16) / 8;
   // (A LOOK-AHEAD form -- warp 0 finishes row tile jb + 1 alone and factors the NEXT diagonal block while the other warps work through
-  // block column jb, one barrier per step -- was built and measured: numeric phase 28.30 vs 27.96 ms at C5 B = 512, i.e. no gain: with
+  // block column jb, one barrier per step -- was built and gave no gain: with
   // <= 1 tile pair per warp the step is bound by tile -> diagonal block -> tile, look-ahead or not.  Removed; git history has it.)
   for (int jb = 0; jb < nbk; jb++) {
     if (warp == 0) front_diag_block(PN, ldp, jb, Wd, lane, w, f_first, a.info + item);
@@ -649,8 +649,7 @@ __global__ void __launch_bounds__(THREADS) front_forward_kernel(FrontSolveArgs a
       if (lane < cw) u[k0 + lane] = ui;
     }
     __syncthreads();
-    // rows below the chunk, one row per thread: its 32 consecutive doubles are two cache lines, read once from DRAM (the variant with
-    // G lanes per row and a shuffle reduction measured 5-30 % slower: profiles/README_r02.md)
+    // rows below the chunk, one row per thread: its 32 consecutive doubles are two cache lines, read once from DRAM
     for (int i = k0 + cw + tid; i < r; i += THREADS) {
       const double* row = Lg + (int64_t)i * w + k0;
       double s = 0.0;
@@ -702,7 +701,7 @@ __global__ void __launch_bounds__(THREADS) front_backward_kernel(FrontSolveArgs 
     }
     double acc = 0.0;
     if (rg < RG) {
-      // four loads in flight per thread, summed in row order (the un-unrolled loop had one: ncu, 68 % of the samples on its load)
+      // four loads in flight per thread, summed in row order
       const double* col = Lg + k0 + kk;
       int i = k0 + cw + rg;
       for (; i + 3 * RG < r; i += 4 * RG) {

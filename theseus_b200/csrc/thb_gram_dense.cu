@@ -1,4 +1,4 @@
-// Dense batched Gram  AtA[b] = A[b]^T A[b]  (fp64) for GENUINELY dense Jacobians, sm_100a: TMA-staged tiles + the FP64 tensor pipe.
+// Dense batched Gram  AtA[b] = A[b]^T A[b]  (fp64) for GENUINELY dense Jacobians, sm_90a: TMA-staged tiles + the FP64 tensor pipe.
 //
 // Replaces `At.bmm(A)` of theseus/optimizer/dense_linearization.py:58-62 for cost functions whose Jacobian is dense (AutoDiffCostFunction
 // with dim >> dof: the block-sparse Gram of thb_gram.cu covers pose graphs / bundle adjustment, where A is 99 % structural zeros).
@@ -7,7 +7,7 @@
 //     swizzle; rows / columns past the matrix are zero-filled by the TMA unit, so ragged m and n need no special case in the main loop.
 //   * CTA = one 64 x 64 tile (i-block, j-block <= i-block) of one item's AtA; 4 warps x (32 x 32) warp tiles; k runs over the m rows in
 //     steps of 32 through a 3-stage ring: thread 0 arms an mbarrier with the stage's byte count and issues cp.async.bulk.tensor for the
-//     two column blocks, everybody waits on the barrier's phase, multiplies (mma.sync m8n8k4 f64: tcgen05 has no fp64 kind) and meets at
+//     two column blocks, everybody waits on the barrier's phase, multiplies (mma.sync m8n8k4 f64: wgmma has no fp64 kind) and meets at
 //     a __syncthreads() before the slot is refilled.
 //   * both operands come from the same rows of A: A-operand  a[i][k] = A[k][i0 + i], B-operand  b[k][j] = A[k][j0 + j].
 //   * the tile is written to (i, j) and mirrored to (j, i): AtA is the full symmetric matrix like the reference's.

@@ -28,7 +28,7 @@ constexpr int LN_WARPS = 4;  // warps per CTA; one warp = 32 batch lanes of one 
 
 // Compile-time fence: every element of x must be in a register here, i.e. all the loads that produce x are issued before any
 // instruction that consumes the fenced values.  Without it the compiler sinks each load next to its FMA and recycles one
-// register, which turns 36-72 independent loads into a chain of dependent memory latencies (measured: 10 us per 6x6 block).
+// register, which turns 36-72 independent loads into a chain of dependent memory latencies.
 template <int N>
 __device__ __forceinline__ void loads_issued(double (&x)[N]) {
 #ifndef THB_SIMT_EMU  // (tests/simt: the same source compiled for the host, one OS thread per CUDA thread)
@@ -302,7 +302,7 @@ struct LaneSolveArgs {
 constexpr int LS_WARPS = 16;  // substitution kernels: the CTA's warps split the block list of ONE column (x 32 batch items)
 
 // s[r] -= sum_c L[r][c] v[c]  (L: DJ x DK row-major at off, v at Y[(pv + c)]).  All loads are issued before the first FMA:
-// written as load-FMA pairs ptxas recycles one register and serialises the 42 loads (measured: 10 us per block).
+// written as load-FMA pairs ptxas recycles one register and serialises the 42 loads.
 template <int DJ, int DK>
 __device__ __forceinline__ void blk_mv(double (&s)[DJ], const double* Fb, int64_t off, const double* Yb, int pv, int64_t Bp) {
   double v[DK], l[DJ * DK];

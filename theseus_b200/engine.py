@@ -204,7 +204,7 @@ class Engine:
             return
         # Some variable was rebound since the tables were built.  The common case inside a training / serving loop is that every
         # tensor still lives where it did (objective.update() + adopt_optim_vars() put the new VALUES into the same pool views and
-        # the caller re-uses its input buffers): compare the device pointers before paying for the rebuild (~10 ms at C2: Python over
+        # the caller re-uses its input buffers): compare the device pointers before paying for the rebuild (Python over
         # every cost function + pageable H2D copies of the pointer tables).
         sig = self._bind_signature(which)
         if sig is not None and sig == self._bind_sig.get(which):
@@ -449,7 +449,7 @@ class Engine:
         """AtA [B,n,n] (block scatter over a zero background), Atb [B,n], diag(AtA) [B,n].
 
         The block pattern of AtA is fixed by the objective's structure and the Gram kernel overwrites every pattern
-        block, so the 8*B*n^2-byte zero fill (4.8 GB, ~1.9 ms at C2) is paid once per buffer, not once per iteration.
+        block, so the 8*B*n^2-byte zero fill (4.8 GB at C2) is paid once per buffer, not once per iteration.
         Nothing downstream writes AtA (the damping is fused into the factorisation's load)."""
         B = self.batch_size
         s = _lib.stream_ptr()

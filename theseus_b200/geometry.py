@@ -21,7 +21,7 @@ from . import _lib
 
 def _require_cuda(t: torch.Tensor, what: str):
     if not t.is_cuda:
-        raise RuntimeError(f"theseus_b200.{what}: tensors must live on a CUDA device (B200); the product has no CPU path")
+        raise RuntimeError(f"theseus_b200.{what}: tensors must live on a CUDA device; the product has no CPU path")
 
 
 # ---- consistency checks of group tensors at construction (theseus/geometry/lie_group_check.py:10-105, manifold.py:44-68,123-146) ----

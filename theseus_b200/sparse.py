@@ -298,7 +298,7 @@ def analyze_py(param_size: np.ndarray, ptrs: np.ndarray, inds: np.ndarray, order
 def _chains(N, struct, parent):
     """Fundamental supernodes ("chains"): maximal runs j, j+1, ... with parent(j) = j+1, struct(j) = {j+1} + struct(j+1) and j the only
     child of j+1.  Returns (chain_of [N]: index of the column's chain, chain_level [num_chains]: level in the chain tree).  Not used by
-    the round-1 kernels; it is the partition the round-2 numeric phase will run on (profiles/r01f_sparse_lane_notes.md)."""
+    the round-1 kernels; it is the partition the round-2 numeric phase will run on."""
     nchild = np.zeros(N, dtype=np.int64)
     for j in range(N):
         if parent[j] >= 0:
@@ -392,10 +392,10 @@ def gram_out_offsets(plan: SparsePlan):
 
 
 def root_split(plan: SparsePlan, max_root_dof: int = 1024, min_root_cols: int = 8):
-    """Round-2 building block (host side, CPU-tested; no kernel consumes it yet -- see profiles/r01f_sparse_lane_notes.md).
+    """Round-2 building block (host side, CPU-tested; no kernel consumes it yet).
 
     The top of the elimination tree is a long chain whose columns form a DENSE trailing block (C5: the last 64 columns, 384 dof):
-    ~200 serial one-column levels for the lane kernels, a < 1 ms job for the dense DMMA Cholesky.  This splits a plan at `cut`:
+    ~200 serial one-column levels for the lane kernels, one small job for the dense DMMA Cholesky.  This splits a plan at `cut`:
       * bottom: columns < cut with the usual per-level lane work lists (their blocks in root ROWS are ordinary blocks of those columns),
       * root assembly: for every root block (i, j), i >= j >= cut, the update pairs that come from bottom columns (k < cut: a prefix
         of the block's pair list) -> S = A_root - sum_k L_ik L_jk^T, copied into a dense [B, nt, nt] matrix and factored there,
@@ -513,7 +513,7 @@ def chain_tiles(plan: SparsePlan, max_width: int = 4, tile_rows: int = 4, breaks
       * external updates run per TILE = (piece, tile_rows consecutive rows of the piece's row structure): the tile's targets are the
         blocks (i, j), i in the row tile, j in the piece, i >= j; for every source column k that updates any of them the tile needs at
         most tile_rows + max_width source blocks L_ik, L_jk -- staged once (shared memory on the GPU) and used by all targets of the
-        tile that have both.  This is where the 1.96 -> 0.70 block loads per update come from (profiles/r01f_sparse_lane_notes.md);
+        tile that have both.  This is where the 1.96 -> 0.70 block loads per update come from;
       * a piece's tiles are due at the level of its first column (all external sources are descendants of j0, hence finished);
         internal updates and the diagonal/triangular stage stay per column and per level as today.
 
