@@ -736,9 +736,11 @@ __global__ void __launch_bounds__(THREADS) front_backward_kernel(FrontSolveArgs 
 
 static inline int front_threads_of_class(int cls) { return cls == 0 ? 64 : (cls == 1 ? 128 : 256); }
 
+// Opt in to the launch's dynamic shared memory whenever it grows, not only above 48 KB: the 48 KB default limit also counts the kernel's
+// static shared memory (front_assemble_kernel's children descriptors), so a launch of exactly 48 KB -- a big front with np = 384 -- failed.
 template <typename K>
 static inline int front_set_smem(K kernel, size_t bytes, size_t* cache) {
-  if (bytes > 48 * 1024 && bytes > *cache) {
+  if (bytes > *cache) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return (int)e;
     *cache = bytes;
