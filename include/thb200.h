@@ -481,6 +481,20 @@ int thb_front_factor_f64(const thb_front_plan* p, const int64_t* launches, int64
 /* x = (L L^T)^-1 rhs; rhs, x [B, n] in ORIGINAL column order; work [B, n], varena [2, B, varena_size] scratch */
 int thb_front_solve_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, const double* factor, const double* rhs,
                         double* x, double* work, double* varena, int64_t B, thb_stream_t stream);
+/* thb_front_factor_f64 + the forward substitution y = L^-1 rhs in the same pass: each shared-memory front runs it on its panel while the
+ * panel is still on chip (no second read of L); rhs [B, n] in ORIGINAL column order, y -> work [B, n] (permuted order), varena
+ * [2, B, varena_size] scratch.  y and the factor are bitwise those of thb_front_factor_f64 + the forward pass of thb_front_solve_f64. */
+int thb_front_factor_forward_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, double* factor, const double* ata,
+                                 int64_t ata_stride, const double* alpha, const double* beta, double* arena, void* dense_ws,
+                                 int64_t dense_ws_bytes, int32_t* info, const double* rhs, double* work, double* varena, int64_t B,
+                                 thb_stream_t stream);
+/* the forward substitution alone: y = L^-1 rhs -> work (permuted order); the first half of thb_front_solve_f64 */
+int thb_front_forward_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, const double* factor, const double* rhs,
+                          double* work, double* varena, int64_t B, thb_stream_t stream);
+/* the backward substitution alone: x = L^-T y with y in work (left there by thb_front_factor_forward_f64); x [B, n] in ORIGINAL column
+ * order, work receives x in permuted order */
+int thb_front_backward_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, const double* factor, double* x,
+                           double* work, int64_t B, thb_stream_t stream);
 int64_t thb_potrf_partial_workspace_bytes(int64_t B, int64_t np);
 int thb_potrf_partial_inplace_f64(double* F, int64_t bstride, int64_t np, int32_t nb_piv, int32_t w_real, int32_t n_real, int32_t info_base,
                                   int32_t* info, int64_t B, void* workspace, int64_t workspace_bytes, thb_stream_t stream);

@@ -144,6 +144,10 @@ SIGNATURES = {
     "thb_front_small_smem_bytes": (c_i64, [c_i32, c_i32, c_i32]),
     "thb_front_factor_f64": (c_i32, [_PF, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "thb_front_solve_f64": (c_i32, [_PF, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "thb_front_factor_forward_f64": (c_i32, [_PF, c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp,
+                                             c_i64, c_vp]),
+    "thb_front_forward_f64": (c_i32, [_PF, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
+    "thb_front_backward_f64": (c_i32, [_PF, c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_vp]),
     "thb_potrf_partial_workspace_bytes": (c_i64, [c_i64, c_i64]),
     "thb_potrf_partial_inplace_f64": (c_i32, [c_vp, c_i64, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "thb_solve_backward_f64": (c_i32, [c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp, c_vp, c_vp]),

@@ -84,9 +84,13 @@ struct FrontArgs {
   double* arena_cur;        // [B, arena_size] of this depth's parity
   const double* arena_child;
   int32_t* info;
-  int prefetch;             // ask L2 for the children's update matrices at kernel start (THB_FRONT_PREFETCH=0 switches it off: A/B runs)
+  int prefetch;             // ask L2 for the children's update matrices at kernel start (THB_FRONT_PREFETCH=1; off by default: slower on H100)
   const double* ata;        // [B, ata_stride] compact AtA blocks (thb_gram_f64 with the plan's compact offsets), or null: the panels
   int64_t ata_stride;       //   in `factor` already hold AtA (zero-filled + scattered by the caller: the extlib-style flow)
+  const double* rhs;        // [B, n] original order, or null: factor only.  Else the forward substitution of every front runs on its
+  double* work;             //   panel while it is still in shared memory: y of the pivots -> work [B, n] (permuted order),
+  double* v_cur;            //   the border vector -> v_cur (this depth's parity of the border-vector arena),
+  const double* v_child;    //   the children's border vectors <- v_child (the other parity)
 };
 
 // AtA entry of panel element e of the front whose panel starts at `poff`: through the plan's panel map when the compact block storage
@@ -218,8 +222,81 @@ __device__ __forceinline__ void front_tile_column(double* PN, int ldp, int jb, i
 
 struct FrontChild {       // one child of the front this CTA works on (shared memory, <= FRONT_MAX_CHILDREN)
   const double* src;      // its update matrix for this item
-  int ldg, lo, hi, pad;   // leading dimension; range [lo, hi] of this front's rows the child reaches
+  int ldg, lo, hi, uoff;  // leading dimension; range [lo, hi] of this front's rows the child reaches; its border vector's offset (f_u_off)
 };
+
+// ------------------------------------------------------------------------------------------------ forward elimination of one front
+// One warp: solve T y = u (lower triangular cw x cw, row stride ld) -- lane i owns u_i
+__device__ __forceinline__ double front_warp_trsv_lower(const double* T, int ld, double ui, int cw, int lane) {
+  const double rd = lane < cw ? 1.0 / T[lane * ld + lane] : 0.0;
+  for (int k = 0; k < cw; k++) {
+    const double yk = __shfl_sync(0xffffffffu, ui * rd, k);
+    if (lane == k) ui = yk;
+    else if (lane > k && lane < cw) ui -= T[lane * ld + k] * yk;
+  }
+  return ui;
+}
+
+// Rows of L as the substitution kernel reads them: the factor in global memory (row-major, stride w), each 32 x 32 diagonal block
+// staged in T [32][33] before its triangular solve
+struct FrontRowsGlobal {
+  static constexpr bool kInPanel = false;
+  const double* L;
+  int w;
+  double* T;
+  __device__ __forceinline__ const double* row(int i) const { return L + (int64_t)i * w; }
+  __device__ __forceinline__ const double* diag(int k0, int cw, int tid, int nthreads, int* ld) const {
+    for (int e = tid; e < cw * cw; e += nthreads) {
+      const int i = e / cw, j = e - i * cw;
+      T[i * 33 + j] = L[(int64_t)(k0 + i) * w + k0 + j];
+    }
+    *ld = 33;
+    return T;
+  }
+};
+// ... and as the factor kernel reads them: in place in its shared-memory panel (row stride ldp, border rows shifted by w8 - w)
+struct FrontRowsPanel {
+  static constexpr bool kInPanel = true;
+  const double* PN;
+  int ldp, w, shift;
+  __device__ __forceinline__ const double* row(int i) const { return PN + (i < w ? i : i + shift) * ldp; }
+  __device__ __forceinline__ const double* diag(int k0, int, int, int, int* ld) const {
+    *ld = ldp;
+    return PN + k0 * ldp + k0;
+  }
+};
+
+// CTA: u <- L^-1 u over the w pivot columns of a front of r rows, 32 columns at a time (u[i] at u[i * us]): a one-warp
+// triangular solve on the chunk's diagonal block, then one row per thread for the rows below it.  The border part of u ends as
+// u_b - P y.  Both the substitution kernel and the fused factor kernel run this same code (each row's sum in the same order whichever
+// thread owns it), so their y and border vectors are bitwise equal.
+template <int THREADS, typename Rows>
+__device__ __forceinline__ void front_forward_elim(const Rows& R, double* u, int us, int w, int r, int tid, int lane) {
+  for (int k0 = 0; k0 < w; k0 += 32) {
+    const int cw = min(32, w - k0);
+    int ld;
+    const double* T = R.diag(k0, cw, tid, THREADS, &ld);
+    __syncthreads();
+    if (tid < 32) {
+      const double ui = front_warp_trsv_lower(T, ld, lane < cw ? u[(k0 + lane) * us] : 0.0, cw, lane);
+      if (lane < cw) u[(k0 + lane) * us] = ui;
+    }
+    __syncthreads();
+    // rows below the chunk, one row per thread (from global memory: its 32 consecutive doubles are two cache lines, read once from DRAM)
+    for (int i = k0 + cw + tid; i < r; i += THREADS) {
+      const double* row = R.row(i) + k0;
+      double s = 0.0;
+      if constexpr (Rows::kInPanel) {
+#pragma unroll 2   // the factor kernel's 64 registers: a deeper unroll spills
+        for (int k = 0; k < cw; k++) s += row[k] * u[(k0 + k) * us];
+      } else {
+        for (int k = 0; k < cw; k++) s += row[k] * u[(k0 + k) * us];
+      }
+      u[i * us] -= s;
+    }
+    __syncthreads();
+  }
+}
 
 // Registers are capped at 64 per thread (1 024 threads per SM): the kernel is bound by the latency chain of a CTA, so resident warps count.
 template <int THREADS>
@@ -241,7 +318,6 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
   const int f_cb_ld = (int)FD[6];
   const int c_begin = (int)(FD[7] & 0xffffffffLL);
   const int nch = min((int)(FD[7] >> 32), FRONT_MAX_CHILDREN);
-  (void)t;
   const int b16 = (b + 15) & ~15, w8 = (w + 7) & ~7;
   const int ldp = front_pad_ld(w8);
   const int prow = w8 + b16 + 8;
@@ -259,6 +335,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
       ch[q].ldg = cld;
       ch[q].lo = (int)PC[2];
       ch[q].hi = (int)PC[3];
+      ch[q].uoff = (int)PC[5];
     }
     const int32_t* inv = p.c_inv + PC[4];
     for (int l = tid; l < r; l += THREADS) INV[q * r + l] = inv[l];
@@ -267,8 +344,18 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
   for (int e = tid; e < prow * ldp; e += THREADS) sm[e] = 0.0;
   THB_PDL_WAIT();   // everything above reads the plan only; below: the children's update matrices, AtA, and every global write
 #ifndef THB_SIMT_EMU
+  // forward substitution: the right-hand side of the pivots (through the permutation) and the children's border vectors are read once
+  // the panel is assembled; ask L2 for them now (measured on H100: the fused substitution costs ~2 ms less per solve of C5 at batch 2048)
+  if (a.rhs != nullptr) {
+    for (int i = tid; i < w; i += THREADS) asm volatile("prefetch.global.L2 [%0];\n" ::"l"(a.rhs + item * p.n + p.perm[f_first + i]));
+    for (int q = 0; q < nch; q++) {
+      const int64_t* PC = p.pc + (int64_t)(c_begin + q) * 6;
+      const double* cu = a.v_child + item * p.varena_size + PC[5];
+      for (int off = tid * 16; off < (int)(PC[1] >> 32); off += THREADS * 16) asm volatile("prefetch.global.L2 [%0];\n" ::"l"(cu + off));
+    }
+  }
   // the children's update matrices (lower triangles) are read element by element by the gathers below: ask L2 for their lines now, so that
-  // the gathers find them on chip (fire and forget: no register, no stall)
+  // the gathers find them on chip (fire and forget: no register, no stall; opt-in, THB_FRONT_PREFETCH=1)
   for (int q = 0; a.prefetch != 0 && q < nch; q++) {
     const int64_t* PC = p.pc + (int64_t)(c_begin + q) * 6;
     const double* csrc = a.arena_child + item * p.arena_size + PC[0];
@@ -318,6 +405,22 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
         if (ii[u] >= 0) PN[(ii[u] < w ? ii[u] : ii[u] + (w8 - w)) * ldp + jj[u]] = v[u];
     }
   }
+  // forward substitution (a.rhs != null): u lives in column w8 of the panel (u[i] at U[i * ldp]), which neither the factorisation nor the
+  // update-matrix tiles read (their columns stop at w8; ldp >= w8 + 4): no shared memory beyond the panel's.  u = [rhs of the pivots; 0]
+  // + the children's border vectors, gathered through the inverse maps in list order -- front_forward_kernel's order
+  double* U = PN + w8;
+  if (a.rhs != nullptr) {
+    for (int i = tid; i < r; i += THREADS) {
+      double v = i < w ? a.rhs[item * p.n + p.perm[f_first + i]] : 0.0;
+      for (int q = 0; q < nch; q++) {
+        if (i >= ch[q].lo && i <= ch[q].hi) {
+          const int k = INV[q * r + i];
+          if (k >= 0) v += a.v_child[item * p.varena_size + ch[q].uoff + k];
+        }
+      }
+      U[i * ldp] = v;
+    }
+  }
   __syncthreads();
   // ---- blocked left-looking factorisation of the panel, 8 columns at a time ----
   const int nbk = w8 / 8, nrt = (w8 + b16) / 8;
@@ -340,6 +443,13 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
       i += di; j += dj;
       if (j >= w) { j -= w; i++; }
     }
+  }
+  // ---- forward substitution on the factored panel, still in shared memory: y -> work, the border vector -> the parent ----
+  if (a.rhs != nullptr) {
+    front_forward_elim<THREADS>(FrontRowsPanel{PN, ldp, w, w8 - w}, U, ldp, w, r, tid, lane);
+    for (int i = tid; i < w; i += THREADS) a.work[item * p.n + f_first + i] = U[i * ldp];
+    double* ub = a.v_cur + item * p.varena_size + p.f_u_off[t];
+    for (int i = tid; i < b; i += THREADS) ub[i] = U[(w + i) * ldp];
   }
   if (b == 0) return;
   // ---- update matrix: per 16 x 16 tile of the lower triangle  C = gathered children - P_I P_J^T, written once from registers ----
@@ -581,17 +691,7 @@ struct FrontSolveArgs {
                             // every later read is on chip; larger panels are streamed chunk by chunk from global memory
 };
 
-// One warp: solve T y = u (lower triangular cw x cw, row stride 33) -- lane i owns u_i
-__device__ __forceinline__ double front_warp_trsv_lower(const double* T, double ui, int cw, int lane) {
-  const double rd = lane < cw ? 1.0 / T[lane * 33 + lane] : 0.0;
-  for (int k = 0; k < cw; k++) {
-    const double yk = __shfl_sync(0xffffffffu, ui * rd, k);
-    if (lane == k) ui = yk;
-    else if (lane > k && lane < cw) ui -= T[lane * 33 + k] * yk;
-  }
-  return ui;
-}
-// One warp: solve T^T x = t
+// One warp: solve T^T x = t (upper triangular cw x cw, row stride 33) -- the forward direction is front_warp_trsv_lower above
 __device__ __forceinline__ double front_warp_trsv_upper(const double* T, double ti, int cw, int lane) {
   const double rd = lane < cw ? 1.0 / T[lane * 33 + lane] : 0.0;
   for (int k = cw - 1; k >= 0; k--) {
@@ -606,7 +706,7 @@ template <int THREADS>
 __global__ void __launch_bounds__(THREADS) front_forward_kernel(FrontSolveArgs a) {
   extern __shared__ double sm[];
   const thb_front_plan& p = a.p;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31;
   const int64_t item = blockIdx.x;
   THB_PDL_TRIGGER();
   const int64_t* FD = p.fd + (int64_t)(a.s0 + blockIdx.y) * 8;   // flat descriptor of the front (frontal.py)
@@ -637,27 +737,7 @@ __global__ void __launch_bounds__(THREADS) front_forward_kernel(FrontSolveArgs a
     }
   }
   __syncthreads();
-  for (int k0 = 0; k0 < w; k0 += 32) {
-    const int cw = min(32, w - k0);
-    for (int e = tid; e < cw * cw; e += THREADS) {
-      const int i = e / cw, j = e - i * cw;
-      T[i * 33 + j] = Lg[(int64_t)(k0 + i) * w + k0 + j];
-    }
-    __syncthreads();
-    if (warp == 0) {
-      const double ui = front_warp_trsv_lower(T, lane < cw ? u[k0 + lane] : 0.0, cw, lane);
-      if (lane < cw) u[k0 + lane] = ui;
-    }
-    __syncthreads();
-    // rows below the chunk, one row per thread: its 32 consecutive doubles are two cache lines, read once from DRAM
-    for (int i = k0 + cw + tid; i < r; i += THREADS) {
-      const double* row = Lg + (int64_t)i * w + k0;
-      double s = 0.0;
-      for (int k = 0; k < cw; k++) s += row[k] * u[k0 + k];
-      u[i] -= s;
-    }
-    __syncthreads();
-  }
+  front_forward_elim<THREADS>(FrontRowsGlobal{Lg, w, T}, u, 1, w, r, tid, lane);
   for (int i = tid; i < w; i += THREADS) a.work[item * p.n + first + i] = u[i];
   if (b > 0) {
     double* ub = a.v_cur + item * p.varena_size + p.f_u_off[t];
@@ -748,15 +828,51 @@ static inline int front_set_smem(K kernel, size_t bytes, size_t* cache) {
   return 0;
 }
 
-}  // namespace thb
+// One launch entry of the substitutions: pass 0 = forward (front_forward_kernel: y -> work, border vectors through varena), pass 1 =
+// backward (front_backward_kernel: work -> x).  Forward launches go deepest first, backward ones roots first.
+static int front_solve_launch(const thb_front_plan* p, const int64_t* L, int pass, const double* factor, const double* rhs, double* x,
+                              double* work, double* varena, int64_t B, cudaStream_t cs) {
+  static size_t fw_set[3] = {0, 0, 0}, bw_set[3] = {0, 0, 0};
+  // tuning knob: largest panel (doubles) the substitution kernels stage in shared memory
+  static const int64_t stage_cap = [] { const char* e = getenv("THB_SOLVE_STAGE"); return e != nullptr ? (int64_t)atoll(e) : (int64_t)0; }();
+  const int depth = (int)L[0], cls = (int)L[1], begin = (int)L[2], count = (int)L[3];
+  FrontSolveArgs a;
+  a.p = *p; a.s0 = begin; a.B = B; a.factor = factor; a.rhs = rhs; a.x = x; a.work = work;
+  a.v_cur = varena != nullptr ? varena + (int64_t)(depth & 1) * B * p->varena_size : nullptr;
+  a.v_child = varena != nullptr ? varena + (int64_t)((depth + 1) & 1) * B * p->varena_size : nullptr;
+  // (merging the launches of a depth into one was measured: slower -- small fronts on 256-thread CTAs)
+  const int kc = cls > 2 ? 2 : cls;
+  const int threads = front_threads_of_class(kc);
+  const int64_t r_max = L[5];   // largest front of the launch (class-3 launches carry np >= r)
+  // panels up to 40 KB are staged on chip (L[6] = largest r * w of a shared-memory launch; class-3 launches stream)
+  const int64_t stage = (cls < 3 && L[6] > 0) ? (L[6] < stage_cap ? L[6] : stage_cap) : 0;
+  a.stage_doubles = (int)stage;
+  const size_t smem = (size_t)(((r_max + 1) & ~1LL) + 32 * 33 + 1 + threads + 2 + stage + 2) * 8;
+  const dim3 grid((unsigned)B, (unsigned)count);
+  if (pass == 0) {
+    if (kc == 0) { int rc = front_set_smem(front_forward_kernel<64>, smem, &fw_set[0]); if (rc) return rc;
+                   FRONT_LAUNCH(front_forward_kernel<64>, grid, 64, smem, cs, a); }
+    else if (kc == 1) { int rc = front_set_smem(front_forward_kernel<128>, smem, &fw_set[1]); if (rc) return rc;
+                        FRONT_LAUNCH(front_forward_kernel<128>, grid, 128, smem, cs, a); }
+    else { int rc = front_set_smem(front_forward_kernel<256>, smem, &fw_set[2]); if (rc) return rc;
+           FRONT_LAUNCH(front_forward_kernel<256>, grid, 256, smem, cs, a); }
+  } else {
+    if (kc == 0) { int rc = front_set_smem(front_backward_kernel<64>, smem, &bw_set[0]); if (rc) return rc;
+                   FRONT_LAUNCH(front_backward_kernel<64>, grid, 64, smem, cs, a); }
+    else if (kc == 1) { int rc = front_set_smem(front_backward_kernel<128>, smem, &bw_set[1]); if (rc) return rc;
+                        FRONT_LAUNCH(front_backward_kernel<128>, grid, 128, smem, cs, a); }
+    else { int rc = front_set_smem(front_backward_kernel<256>, smem, &bw_set[2]); if (rc) return rc;
+           FRONT_LAUNCH(front_backward_kernel<256>, grid, 256, smem, cs, a); }
+  }
+  THB_CHECK_LAUNCH();
+  return THB_OK;
+}
 
-extern "C" {
-
-int64_t thb_front_small_smem_bytes(int32_t w, int32_t b, int32_t nchildren) { return thb::front_smem_doubles(w, b, nchildren) * 8; }
-
-int thb_front_factor_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, double* factor, const double* ata,
-                         int64_t ata_stride, const double* alpha, const double* beta, double* arena, void* dense_ws, int64_t dense_ws_bytes,
-                         int32_t* info, int64_t B, thb_stream_t stream) {
+// The numeric factorisation; with rhs != null also the forward substitution: fused into front_small_kernel for the shared-memory
+// fronts, front_forward_kernel right after the extraction of a big front's panel.
+static int front_factor(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, double* factor, const double* ata,
+                        int64_t ata_stride, const double* alpha, const double* beta, double* arena, void* dense_ws, int64_t dense_ws_bytes,
+                        int32_t* info, const double* rhs, double* work, double* varena, int64_t B, thb_stream_t stream) {
   if (p == nullptr || launches == nullptr || factor == nullptr || arena == nullptr || info == nullptr || B < 0) return THB_ERR_BAD_ARG;
   if (B == 0 || p->S == 0) return THB_OK;
   if (B > 65535LL * 32768LL) return THB_ERR_UNSUPPORTED;
@@ -769,17 +885,24 @@ int thb_front_factor_f64(const thb_front_plan* p, const int64_t* launches, int64
   static int front_prefetch_flag = -1;
   if (front_prefetch_flag < 0) {
     const char* e = getenv("THB_FRONT_PREFETCH");
-    front_prefetch_flag = (e != nullptr && e[0] == '0') ? 0 : 1;
+    // opt-in: on H100 (C5, batch 2048) the prefetch made the factorisation slower, 175 -> 166 ms without it
+    front_prefetch_flag = (e != nullptr && e[0] == '1') ? 1 : 0;
   }
+  // largest CTA of front_small_kernel that runs the forward substitution itself (THB_FRONT_FUSE_MAX: 0 | 64 | ... | 1024); launches of
+  // larger CTAs are followed by front_forward_kernel instead
+  static const int fuse_max = [] { const char* e = getenv("THB_FRONT_FUSE_MAX"); return e != nullptr ? atoi(e) : 1024; }();
   for (int64_t l = 0; l < num_launches; l++) {
     const int64_t* L = launches + l * THB_FRONT_LAUNCH_COLS;
     const int depth = (int)L[0], cls = (int)L[1], begin = (int)L[2], count = (int)L[3];
-    thb::FrontArgs a;
+    FrontArgs a;
     a.p = *p; a.s0 = begin; a.B = B; a.factor = factor; a.alpha = alpha; a.beta = beta; a.info = info;
     a.ata = (ata != nullptr && p->pmap != nullptr) ? ata : nullptr; a.ata_stride = ata_stride;
     a.prefetch = front_prefetch_flag;
     a.arena_cur = arena + (int64_t)(depth & 1) * B * p->arena_size;
     a.arena_child = arena + (int64_t)((depth + 1) & 1) * B * p->arena_size;
+    a.rhs = rhs; a.work = work;
+    a.v_cur = rhs != nullptr ? varena + (int64_t)(depth & 1) * B * p->varena_size : nullptr;
+    a.v_child = rhs != nullptr ? varena + (int64_t)((depth + 1) & 1) * B * p->varena_size : nullptr;
     if (cls < 3) {
       const size_t smem = (size_t)L[4];
 #ifndef THB_SIMT_EMU
@@ -787,23 +910,32 @@ int thb_front_factor_f64(const thb_front_plan* p, const int64_t* launches, int64
 #endif
       const dim3 grid((unsigned)B, (unsigned)count);
       if (count > 65535) return THB_ERR_UNSUPPORTED;
-      if (cls == 0 && thr_cls[0] == 64) {
-        int rc = thb::front_set_smem(thb::front_small_kernel<64>, smem, &smem_set[0]); if (rc) return rc;
-        FRONT_LAUNCH(thb::front_small_kernel<64>, grid, 64, smem, cs, a);
-      } else if ((cls == 0 && thr_cls[0] == 128) || (cls == 1 && thr_cls[1] == 128)) {
-        int rc = thb::front_set_smem(thb::front_small_kernel<128>, smem, &smem_set[1]); if (rc) return rc;
-        FRONT_LAUNCH(thb::front_small_kernel<128>, grid, 128, smem, cs, a);
-      } else if (cls <= 1 || smem <= 56 * 1024) {   // class 2 (> 96 rows): threads so that ~32 warps are resident whatever the panel size
-        int rc = thb::front_set_smem(thb::front_small_kernel<256>, smem, &smem_set[2]); if (rc) return rc;
-        FRONT_LAUNCH(thb::front_small_kernel<256>, grid, 256, smem, cs, a);
-      } else if (smem <= 113 * 1024) {
-        int rc = thb::front_set_smem(thb::front_small_kernel<512>, smem, &smem_set[3]); if (rc) return rc;
-        FRONT_LAUNCH(thb::front_small_kernel<512>, grid, 512, smem, cs, a);
+      const int threads = (cls == 0 && thr_cls[0] == 64) ? 64
+                          : ((cls == 0 && thr_cls[0] == 128) || (cls == 1 && thr_cls[1] == 128)) ? 128
+                          : (cls <= 1 || smem <= 56 * 1024) ? 256 : (smem <= 113 * 1024 ? 512 : 1024);
+      const bool fused = rhs != nullptr && threads <= fuse_max;
+      if (!fused) a.rhs = nullptr;
+      if (threads == 64) {
+        int rc = front_set_smem(front_small_kernel<64>, smem, &smem_set[0]); if (rc) return rc;
+        FRONT_LAUNCH(front_small_kernel<64>, grid, 64, smem, cs, a);
+      } else if (threads == 128) {
+        int rc = front_set_smem(front_small_kernel<128>, smem, &smem_set[1]); if (rc) return rc;
+        FRONT_LAUNCH(front_small_kernel<128>, grid, 128, smem, cs, a);
+      } else if (threads == 256) {   // class 2 (> 96 rows): threads so that ~32 warps are resident whatever the panel size
+        int rc = front_set_smem(front_small_kernel<256>, smem, &smem_set[2]); if (rc) return rc;
+        FRONT_LAUNCH(front_small_kernel<256>, grid, 256, smem, cs, a);
+      } else if (threads == 512) {
+        int rc = front_set_smem(front_small_kernel<512>, smem, &smem_set[3]); if (rc) return rc;
+        FRONT_LAUNCH(front_small_kernel<512>, grid, 512, smem, cs, a);
       } else {                          // one CTA per SM: all 1 024 threads
-        int rc = thb::front_set_smem(thb::front_small_kernel<1024>, smem, &smem_set[4]); if (rc) return rc;
-        FRONT_LAUNCH(thb::front_small_kernel<1024>, grid, 1024, smem, cs, a);
+        int rc = front_set_smem(front_small_kernel<1024>, smem, &smem_set[4]); if (rc) return rc;
+        FRONT_LAUNCH(front_small_kernel<1024>, grid, 1024, smem, cs, a);
       }
       THB_CHECK_LAUNCH();
+      if (rhs != nullptr && !fused) {
+        const int rc = front_solve_launch(p, L, 0, factor, rhs, nullptr, work, varena, B, cs);
+        if (rc != THB_OK) return rc;
+      }
     } else {
       const int64_t np = L[5], nb_piv = L[6], fr_off = L[7], first = L[8];
       const int t = (int)L[9];
@@ -812,20 +944,46 @@ int thb_front_factor_f64(const thb_front_plan* p, const int64_t* launches, int64
       return THB_ERR_UNSUPPORTED;   // the DMMA dense kernel is not part of the host emulation
 #else
       if (dense_ws == nullptr || np % 128 != 0 || np > 8192) return THB_ERR_BAD_ARG;
-      const size_t smem = (size_t)thb::ASM_ROWS * np * 8;
-      int rc = thb::front_set_smem(thb::front_assemble_kernel, smem, &asm_set); if (rc) return rc;
-      thb::front_assemble_kernel<<<dim3((unsigned)B, (unsigned)(np / thb::ASM_ROWS)), thb::ASM_THREADS, smem, cs>>>(a, t);
+      const size_t smem = (size_t)ASM_ROWS * np * 8;
+      int rc = front_set_smem(front_assemble_kernel, smem, &asm_set); if (rc) return rc;
+      front_assemble_kernel<<<dim3((unsigned)B, (unsigned)(np / ASM_ROWS)), ASM_THREADS, smem, cs>>>(a, t);
       THB_CHECK_LAUNCH();
       // w_real / n_real: the k loops stop at the real pivot columns, trailing tiles that lie in the padding are skipped
       rc = thb_potrf_partial_inplace_f64(a.arena_cur + fr_off, p->arena_size, np, (int32_t)nb_piv, (int32_t)L[10], (int32_t)(nb_piv * 64 + L[11]),
                                          (int32_t)first, info, B, dense_ws, dense_ws_bytes, stream);
       if (rc != THB_OK) return rc;
-      thb::front_extract_kernel<<<dim3((unsigned)B, 8), 256, 0, cs>>>(a, t);
+      front_extract_kernel<<<dim3((unsigned)B, 8), 256, 0, cs>>>(a, t);
       THB_CHECK_LAUNCH();
+      if (rhs != nullptr) {   // the panel is in global memory now: the substitution kernel's forward launch for this front
+        rc = front_solve_launch(p, L, 0, factor, rhs, nullptr, work, varena, B, cs);
+        if (rc != THB_OK) return rc;
+      }
 #endif
     }
   }
   return THB_OK;
+}
+
+}  // namespace thb
+
+extern "C" {
+
+int64_t thb_front_small_smem_bytes(int32_t w, int32_t b, int32_t nchildren) { return thb::front_smem_doubles(w, b, nchildren) * 8; }
+
+int thb_front_factor_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, double* factor, const double* ata,
+                         int64_t ata_stride, const double* alpha, const double* beta, double* arena, void* dense_ws, int64_t dense_ws_bytes,
+                         int32_t* info, int64_t B, thb_stream_t stream) {
+  return thb::front_factor(p, launches, num_launches, factor, ata, ata_stride, alpha, beta, arena, dense_ws, dense_ws_bytes, info, nullptr,
+                           nullptr, nullptr, B, stream);
+}
+
+int thb_front_factor_forward_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, double* factor, const double* ata,
+                                 int64_t ata_stride, const double* alpha, const double* beta, double* arena, void* dense_ws,
+                                 int64_t dense_ws_bytes, int32_t* info, const double* rhs, double* work, double* varena, int64_t B,
+                                 thb_stream_t stream) {
+  if (rhs == nullptr || work == nullptr || varena == nullptr) return THB_ERR_BAD_ARG;
+  return thb::front_factor(p, launches, num_launches, factor, ata, ata_stride, alpha, beta, arena, dense_ws, dense_ws_bytes, info, rhs, work,
+                           varena, B, stream);
 }
 
 int thb_front_solve_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, const double* factor, const double* rhs,
@@ -834,45 +992,32 @@ int thb_front_solve_f64(const thb_front_plan* p, const int64_t* launches, int64_
       B < 0)
     return THB_ERR_BAD_ARG;
   if (B == 0 || p->S == 0) return THB_OK;
+  const int rc = thb_front_forward_f64(p, launches, num_launches, factor, rhs, work, varena, B, stream);
+  if (rc != THB_OK) return rc;
+  return thb_front_backward_f64(p, launches, num_launches, factor, x, work, B, stream);
+}
+
+int thb_front_forward_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, const double* factor, const double* rhs,
+                          double* work, double* varena, int64_t B, thb_stream_t stream) {
+  if (p == nullptr || launches == nullptr || factor == nullptr || rhs == nullptr || work == nullptr || varena == nullptr || B < 0)
+    return THB_ERR_BAD_ARG;
+  if (B == 0 || p->S == 0) return THB_OK;
   cudaStream_t cs = thb_cs(stream);
-  static size_t fw_set[3] = {0, 0, 0}, bw_set[3] = {0, 0, 0};
-  // tuning knob: largest panel (doubles) the substitution kernels stage in shared memory
-  static const int64_t stage_cap = [] { const char* e = getenv("THB_SOLVE_STAGE"); return e != nullptr ? (int64_t)atoll(e) : (int64_t)0; }();
-  for (int pass = 0; pass < 2; pass++) {
-    for (int64_t q = 0; q < num_launches; q++) {
-      const int64_t l = pass == 0 ? q : num_launches - 1 - q;   // forward: deepest first; backward: roots first
-      const int64_t* L = launches + l * THB_FRONT_LAUNCH_COLS;
-      const int depth = (int)L[0], cls = (int)L[1], begin = (int)L[2], count = (int)L[3];
-      thb::FrontSolveArgs a;
-      a.p = *p; a.s0 = begin; a.B = B; a.factor = factor; a.rhs = rhs; a.x = x; a.work = work;
-      a.v_cur = varena + (int64_t)(depth & 1) * B * p->varena_size;
-      a.v_child = varena + (int64_t)((depth + 1) & 1) * B * p->varena_size;
-      // (merging the launches of a depth into one was measured: slower -- small fronts on 256-thread CTAs)
-      const int kc = cls > 2 ? 2 : cls;
-      const int threads = thb::front_threads_of_class(kc);
-      const int64_t r_max = L[5];   // largest front of the launch (class-3 launches carry np >= r)
-      // panels up to 40 KB are staged on chip (L[6] = largest r * w of a shared-memory launch; class-3 launches stream)
-      const int64_t stage = (cls < 3 && L[6] > 0) ? (L[6] < stage_cap ? L[6] : stage_cap) : 0;
-      a.stage_doubles = (int)stage;
-      const size_t smem = (size_t)(((r_max + 1) & ~1LL) + 32 * 33 + 1 + threads + 2 + stage + 2) * 8;
-      const dim3 grid((unsigned)B, (unsigned)count);
-      if (pass == 0) {
-        if (kc == 0) { int rc = thb::front_set_smem(thb::front_forward_kernel<64>, smem, &fw_set[0]); if (rc) return rc;
-                       FRONT_LAUNCH(thb::front_forward_kernel<64>, grid, 64, smem, cs, a); }
-        else if (kc == 1) { int rc = thb::front_set_smem(thb::front_forward_kernel<128>, smem, &fw_set[1]); if (rc) return rc;
-                            FRONT_LAUNCH(thb::front_forward_kernel<128>, grid, 128, smem, cs, a); }
-        else { int rc = thb::front_set_smem(thb::front_forward_kernel<256>, smem, &fw_set[2]); if (rc) return rc;
-               FRONT_LAUNCH(thb::front_forward_kernel<256>, grid, 256, smem, cs, a); }
-      } else {
-        if (kc == 0) { int rc = thb::front_set_smem(thb::front_backward_kernel<64>, smem, &bw_set[0]); if (rc) return rc;
-                       FRONT_LAUNCH(thb::front_backward_kernel<64>, grid, 64, smem, cs, a); }
-        else if (kc == 1) { int rc = thb::front_set_smem(thb::front_backward_kernel<128>, smem, &bw_set[1]); if (rc) return rc;
-                            FRONT_LAUNCH(thb::front_backward_kernel<128>, grid, 128, smem, cs, a); }
-        else { int rc = thb::front_set_smem(thb::front_backward_kernel<256>, smem, &bw_set[2]); if (rc) return rc;
-               FRONT_LAUNCH(thb::front_backward_kernel<256>, grid, 256, smem, cs, a); }
-      }
-      THB_CHECK_LAUNCH();
-    }
+  for (int64_t q = 0; q < num_launches; q++) {   // deepest first
+    const int rc = thb::front_solve_launch(p, launches + q * THB_FRONT_LAUNCH_COLS, 0, factor, rhs, nullptr, work, varena, B, cs);
+    if (rc != THB_OK) return rc;
+  }
+  return THB_OK;
+}
+
+int thb_front_backward_f64(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, const double* factor, double* x,
+                           double* work, int64_t B, thb_stream_t stream) {
+  if (p == nullptr || launches == nullptr || factor == nullptr || x == nullptr || work == nullptr || B < 0) return THB_ERR_BAD_ARG;
+  if (B == 0 || p->S == 0) return THB_OK;
+  cudaStream_t cs = thb_cs(stream);
+  for (int64_t q = num_launches - 1; q >= 0; q--) {   // roots first
+    const int rc = thb::front_solve_launch(p, launches + q * THB_FRONT_LAUNCH_COLS, 1, factor, nullptr, x, work, nullptr, B, cs);
+    if (rc != THB_OK) return rc;
   }
   return THB_OK;
 }

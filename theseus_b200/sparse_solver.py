@@ -201,7 +201,10 @@ class BaspachoSparseSolver(LinearSolver):
                          max_np=int(big[:, 5].max()) if len(big) else 0)
         return self._dev
 
-    def _numeric_front(self, A_val, b, alpha, beta):
+    def _numeric_front(self, A_val, b, alpha, beta, forward=False):
+        """Gram + factor, chunk by chunk.  forward=True: the forward substitution of A^T b runs inside the factorisation (each
+        front on its panel while the panel is in shared memory, thb_front_factor_forward_f64) and leaves y in bufs['work'];
+        _backward_front() finishes the solve."""
         B, device = A_val.shape[0], A_val.device
         d = self._device_plan(device)
         P = self._plan
@@ -234,11 +237,15 @@ class BaspachoSparseSolver(LinearSolver):
         L = d["launches"]
         for c0 in range(0, B, chunk):
             nb = min(chunk, B - c0)
-            _lib.check(lib.thb_front_factor_f64(
-                C.byref(d["front"]), L.ctypes.data, L.shape[0], _lib.ptr(factor[c0:]), _lib.ptr(ata[c0:]), self._ata_size,
-                _lib.ptr(alpha[c0:]) if alpha is not None else None,
-                _lib.ptr(beta[c0:]) if beta is not None else None, _lib.ptr(bufs["arena"]), _lib.ptr(bufs["ws"]) if d["max_np"] else None,
-                bufs["ws"].numel(), _lib.ptr(info[c0:]), nb, s), "front_factor")
+            args = (C.byref(d["front"]), L.ctypes.data, L.shape[0], _lib.ptr(factor[c0:]), _lib.ptr(ata[c0:]), self._ata_size,
+                    _lib.ptr(alpha[c0:]) if alpha is not None else None,
+                    _lib.ptr(beta[c0:]) if beta is not None else None, _lib.ptr(bufs["arena"]), _lib.ptr(bufs["ws"]) if d["max_np"] else None,
+                    bufs["ws"].numel(), _lib.ptr(info[c0:]))
+            if forward:
+                _lib.check(lib.thb_front_factor_forward_f64(*args, _lib.ptr(Atb[c0:]), _lib.ptr(bufs["work"][c0:]), _lib.ptr(bufs["varena"]), nb, s),
+                           "front_factor_forward")
+            else:
+                _lib.check(lib.thb_front_factor_f64(*args, nb, s), "front_factor")
         self._keep = (A_val, b, alpha, beta)
         return Atb
 
@@ -255,6 +262,20 @@ class BaspachoSparseSolver(LinearSolver):
             _lib.check(lib.thb_front_solve_f64(C.byref(d["front"]), L.ctypes.data, L.shape[0], _lib.ptr(bufs["factor"][c0:]), _lib.ptr(rhs[c0:]),
                                                _lib.ptr(x[c0:]), _lib.ptr(bufs["work"][c0:]), _lib.ptr(bufs["varena"]), nb, _lib.stream_ptr()),
                        "front_solve")
+        return x
+
+    def _backward_front(self):
+        """x = L^-T y, y left in bufs['work'] by _numeric_front(..., forward=True)."""
+        d, P = self._dev, self._plan
+        bufs = d["bufs"]
+        B, chunk = bufs["key"][0], bufs["chunk"]
+        lib = _lib.load()
+        x = torch.empty(B, P.n, dtype=torch.float64, device=bufs["work"].device)
+        L = d["launches"]
+        for c0 in range(0, B, chunk):
+            nb = min(chunk, B - c0)
+            _lib.check(lib.thb_front_backward_f64(C.byref(d["front"]), L.ctypes.data, L.shape[0], _lib.ptr(bufs["factor"][c0:]), _lib.ptr(x[c0:]),
+                                                  _lib.ptr(bufs["work"][c0:]), nb, _lib.stream_ptr()), "front_backward")
         return x
 
     def _lane_struct(self, ln, dev, device):
@@ -308,8 +329,13 @@ class BaspachoSparseSolver(LinearSolver):
         alpha = beta = None
         if damping is not None:
             alpha, beta = convert_to_alpha_beta_damping_tensors(damping, damping_eps, ellipsoidal_damping, A64.shape[0], A64.device, torch.float64)
-        Atb = self._numeric(A64, b64, alpha, beta)
-        x = self._substitute(Atb)
+        if self.layout_for(A64.shape[0]) == "front":
+            # the forward substitution of A^T b rides on the factorisation (no second read of L), then the backward pass
+            self._numeric_front(A64, b64, alpha, beta, forward=True)
+            x = self._backward_front()
+        else:
+            Atb = self._numeric(A64, b64, alpha, beta)
+            x = self._substitute(Atb)
         self._last_info = self._dev["bufs"]["info"]
         if not getattr(self, "defer_info_check", False):  # CUDA-graph capture: no host sync here, check_info() after the replay
             self.check_info()
