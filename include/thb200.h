@@ -52,13 +52,29 @@ enum thb_cost_kind {
   THB_COST_LOCAL_VECTOR = 4, /* Difference on Vector/Point: e = x - target, J = I (geometry/vector.py) */
   THB_COST_BETWEEN_SE2 = 6,  /* Between with SE2 [B,4] = [x,y,cos,sin] (theseus/geometry/se2.py) */
   THB_COST_LOCAL_SE2 = 7,    /* Difference / Local with SE2 */
-  THB_COST_REPROJECTION = 5  /* theseus/embodied/measurements/reprojection.py:54-94: x0 = camera SE3, x1 = Point3,
+  THB_COST_REPROJECTION = 5, /* theseus/embodied/measurements/reprojection.py:54-94: x0 = camera SE3, x1 = Point3,
                                 aux = focal_length [Bf,1], aux2 = image_feature_point [Bi,2], aux3 = calib_k1, aux4 = calib_k2 */
+  /* Motion planning (theseus/embodied/collision/collision.py, motionmodel/double_integrator.py, motionmodel/misc.py).
+   * Collision2D: x0 = pose (Point2 [B,2] / SE2 [B,4]); aux = sdf origin [Bo,2], aux2 = sdf data [Bd,rows,cols],
+   *   aux3 = cell size [Bc,1], aux4 = cost_eps [Be,1]; grid_rows / grid_cols = the grid shape.  e = max(eps - sdf(xy), 0), dim 1. */
+  THB_COST_COLLISION2D_POINT2 = 8,
+  THB_COST_COLLISION2D_SE2 = 9,
+  /* DoubleIntegrator / GPMotionModel: x0 = pose1, x1 = vel1, x2 = pose2, x3 = vel2; aux = dt [Bd,1]; with THB_WEIGHT_GP
+   * aux2 = the weight's dt [Bg,1].  e = [local(pose1, pose2) - dt vel1, vel2 - vel1], dim 2 dof (dof 1..3 for the Vector kind). */
+  THB_COST_DOUBLE_INTEGRATOR_VECTOR = 10,
+  THB_COST_DOUBLE_INTEGRATOR_SE2 = 11,
+  /* HingeCost: x0 = vector [B,dof] (dof 1..3); aux = down_limit, aux2 = up_limit, aux3 = threshold, each [Bl,dof] (limits may be +-inf). */
+  THB_COST_HINGE = 12,
+  /* Nonholonomic: x0 = pose (SE2 [B,4] / Vector [B,3]), x1 = vel [B,3]; dim 1. */
+  THB_COST_NONHOLONOMIC_SE2 = 13,
+  THB_COST_NONHOLONOMIC_VECTOR = 14
 };
 enum thb_robust_kind { THB_ROBUST_NONE = 0, THB_ROBUST_WELSCH = 1, THB_ROBUST_HUBER = 2 };
 enum thb_weight_kind {
-  THB_WEIGHT_SCALE = 0,   /* theseus/core/cost_weight.py:60-93  (ScaleCostWeight, tensor [Bw,1]) */
-  THB_WEIGHT_DIAGONAL = 1 /* theseus/core/cost_weight.py:98-139 (DiagonalCostWeight, tensor [Bw,dim]) */
+  THB_WEIGHT_SCALE = 0,    /* theseus/core/cost_weight.py:60-93  (ScaleCostWeight, tensor [Bw,1]) */
+  THB_WEIGHT_DIAGONAL = 1, /* theseus/core/cost_weight.py:98-139 (DiagonalCostWeight, tensor [Bw,dim]) */
+  THB_WEIGHT_GP = 2        /* embodied/motionmodel/double_integrator.py:94-176 (GPCostWeight): w = Qc_inv [Bq,d,d], dt in aux2;
+                              the weight applied is L^T, L = chol([[12/dt^3, -6/dt^2], [-6/dt^2, 4/dt]] (x) Qc_inv) */
 };
 enum thb_var_kind { THB_VAR_SE3 = 0, THB_VAR_SO3 = 1, THB_VAR_VECTOR = 2, THB_VAR_SE2 = 3, THB_VAR_SO2 = 4 };
 
@@ -91,6 +107,15 @@ typedef struct thb_cost_group {
   int32_t reserved0;
   const void* const* log_radius;
   const int32_t* bstride_lr;
+  /* Cost functions with more than two optimisation variables (DoubleIntegrator): device [K] pointers to the third and fourth
+   * variable, their batch strides in device int32 [K,2] (NULL otherwise).  `bp` is then [K, 4]; it is [K, 2] for every kind with
+   * at most two variables. */
+  const void* const* x2;
+  const void* const* x3;
+  const int32_t* bstride3;
+  /* Collision2D: shape of the SDF grids of the group (every cost function of a group has the same one). */
+  int32_t grid_rows;
+  int32_t grid_cols;
 } thb_cost_group;
 
 /* Fused residual + analytic Jacobian + weighting for every (cost function, batch item) of a group;

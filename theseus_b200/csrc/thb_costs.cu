@@ -33,6 +33,10 @@ template <typename T> struct GroupDev {
   int robust_kind;
   const T* const* log_radius;
   const int32_t* bstride_lr;
+  const T* const* x2;
+  const T* const* x3;
+  const int32_t* bstride3;
+  int grid_rows, grid_cols;
 };
 
 template <typename T> static GroupDev<T> to_dev(const thb_cost_group* g) {
@@ -57,6 +61,11 @@ template <typename T> static GroupDev<T> to_dev(const thb_cost_group* g) {
   d.robust_kind = g->robust_kind;
   d.log_radius = reinterpret_cast<const T* const*>(g->log_radius);
   d.bstride_lr = g->bstride_lr;
+  d.x2 = reinterpret_cast<const T* const*>(g->x2);
+  d.x3 = reinterpret_cast<const T* const*>(g->x3);
+  d.bstride3 = g->bstride3;
+  d.grid_rows = g->grid_rows;
+  d.grid_cols = g->grid_cols;
   return d;
 }
 
@@ -509,6 +518,346 @@ template <typename T> __global__ void error_vector_kernel(GroupDev<T> g, int64_t
   partial[(int64_t)c * B + b] = acc * T(0.5);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Motion-planning cost functions: Collision2D (embodied/collision/collision.py:44-73 + signed_distance_field.py:163-241),
+// DoubleIntegrator / GPMotionModel (motionmodel/double_integrator.py:45-80) with GPCostWeight (:131-170), HingeCost and
+// Nonholonomic (motionmodel/misc.py:62-84, 126-178).  Every optimisation variable of one of these cost functions has the same dof D;
+// a cost function's row block is DIM x (NVARS * D).  The unweighted Jacobian is written straight into the warp's staging area (the
+// layout of A_val), the weight is applied there, and the warp stores the rows with consecutive lanes like linearize_kernel.
+template <typename T> __device__ __forceinline__ T t_floor(T x);
+template <> __device__ __forceinline__ float t_floor<float>(float x) { return floorf(x); }
+template <> __device__ __forceinline__ double t_floor<double>(double x) { return floor(x); }
+
+template <int KIND, int D> struct Mp {
+  static constexpr bool COLL = KIND == THB_COST_COLLISION2D_POINT2 || KIND == THB_COST_COLLISION2D_SE2;
+  static constexpr bool DI = KIND == THB_COST_DOUBLE_INTEGRATOR_VECTOR || KIND == THB_COST_DOUBLE_INTEGRATOR_SE2;
+  static constexpr bool NH = KIND == THB_COST_NONHOLONOMIC_SE2 || KIND == THB_COST_NONHOLONOMIC_VECTOR;
+  static constexpr int DIM = (COLL || NH) ? 1 : (DI ? 2 * D : D);
+  static constexpr int NVARS = DI ? 4 : (NH ? 2 : 1);
+  static constexpr int BPW = NVARS > 2 ? NVARS : 2;   // row length of the group's bp table
+  static constexpr int COLS = NVARS * D;
+  static constexpr int NV = DIM * COLS;
+};
+
+template <typename T> __device__ __forceinline__ const T* mp_var(const GroupDev<T>& g, int v, int k, int64_t b) {
+  if (v == 0) return g.x0[k] + (int64_t)g.bstride[k * 4 + 0] * b;
+  if (v == 1) return g.x1[k] + (int64_t)g.bstride[k * 4 + 1] * b;
+  if (v == 2) return g.x2[k] + (int64_t)g.bstride3[k * 2 + 0] * b;
+  return g.x3[k] + (int64_t)g.bstride3[k * 2 + 1] * b;
+}
+template <typename T> __device__ __forceinline__ const T* mp_aux(const GroupDev<T>& g, int q, int k, int64_t b) {
+  if (q == 0) return g.aux[k] + (int64_t)g.bstride[k * 4 + 2] * b;
+  const T* const* p = (q == 1) ? g.aux2 : ((q == 2) ? g.aux3 : g.aux4);
+  return p[k] + (int64_t)g.bstride2[k * 3 + (q - 1)] * b;
+}
+
+// Unweighted error e[DIM] and (WITH_J) Jacobian rows S[r * stride + bp[v] + c] of one cost function.
+template <typename T, int KIND, int D, bool WITH_J>
+__device__ __forceinline__ void mp_cost(const GroupDev<T>& g, int k, int64_t b, T* e, T* S, int stride, const int* bp) {
+  using M = Mp<KIND, D>;
+  if constexpr (M::COLL) {
+    // sdf by bilinear interpolation, 0 (and a zero gradient) outside the grid; e = max(eps - sdf, 0), J = -d sdf where sdf <= eps
+    const T* x = mp_var(g, 0, k, b);
+    const T px = x[0], py = x[1];
+    const T* org = mp_aux(g, 0, k, b);
+    const T* data = mp_aux(g, 1, k, b);
+    const T cell = mp_aux(g, 2, k, b)[0];
+    const T eps = mp_aux(g, 3, k, b)[0];
+    const int R = g.grid_rows, C = g.grid_cols;
+    const T ox = org[0], oy = org[1];
+    const bool oob = (px < ox) || (px > ox + (T(C) - T(1)) * cell) || (py < oy) || (py > oy + (T(R) - T(1)) * cell);
+    T dist = T(0), jx = T(0), jy = T(0);
+    if (!oob) {
+      const T col = (px - ox) / cell, row = (py - oy) / cell;
+      const T lr = t_floor(row), lc = t_floor(col);
+      const T hr = lr + T(1), hc = lc + T(1);
+      auto clampi = [](T v, int hi) { return !(v >= T(0)) ? 0 : (v > T(hi) ? hi : (int)v); };
+      const int lri = clampi(lr, R - 1), lci = clampi(lc, C - 1), hri = clampi(hr, R - 1), hci = clampi(hc, C - 1);
+      const T g00 = data[(int64_t)lri * C + lci], g10 = data[(int64_t)hri * C + lci];
+      const T g01 = data[(int64_t)lri * C + hci], g11 = data[(int64_t)hri * C + hci];
+      const T hrd = hr - row, hcd = hc - col, lrd = row - lr, lcd = col - lc;
+      dist = hrd * hcd * g00 + lrd * hcd * g10 + hrd * lcd * g01 + lrd * lcd * g11;
+      jx = (hrd * (g01 - g00) + lrd * (g11 - g10)) / cell;
+      jy = (hcd * (g10 - g00) + lcd * (g11 - g01)) / cell;
+    }
+    const T err = eps - dist;
+    e[0] = err < T(0) ? T(0) : err;
+    if (WITH_J) {
+      if (dist > eps) jx = jy = T(0);
+      if (KIND == THB_COST_COLLISION2D_POINT2) {
+        S[bp[0] + 0] = -jx;
+        S[bp[0] + 1] = -jy;
+      } else {   // d xy / d tangent of SE2 = [R | 0] (se2.py:143-150)
+        const T c = x[2], s = x[3];
+        S[bp[0] + 0] = -(jx * c + jy * s);
+        S[bp[0] + 1] = -(jx * -s + jy * c);
+        S[bp[0] + 2] = T(0);
+      }
+    }
+  } else if constexpr (M::DI) {
+    // e = [local(pose1, pose2) - dt vel1, vel2 - vel1]
+    const T* v1 = mp_var(g, 1, k, b);
+    const T* v2 = mp_var(g, 3, k, b);
+    const T dt = mp_aux(g, 0, k, b)[0];
+    T pd[D], J1[D * D], J2[D * D];
+    if constexpr (KIND == THB_COST_DOUBLE_INTEGRATOR_SE2) {
+      T X1[4], X2[4], Dm[4], Jl[9];
+      load_n<T, 4>(mp_var(g, 0, k, b), X1);
+      load_n<T, 4>(mp_var(g, 2, k, b), X2);
+      se2_between(X1, X2, Dm);
+      se2_log_jlog<T, WITH_J>(Dm, pd, Jl);
+      if (WITH_J) {   // local's Jacobians: -dlog Ad(D^-1), dlog (as Between with an identity measurement)
+        T Di[4], Ad[9];
+        se2_inverse(Dm, Di);
+        se2_adjoint(Di, Ad);
+#pragma unroll
+        for (int r = 0; r < 3; r++)
+#pragma unroll
+          for (int c = 0; c < 3; c++) {
+            J1[r * 3 + c] = -(Jl[r * 3 + 0] * Ad[0 * 3 + c] + Jl[r * 3 + 1] * Ad[1 * 3 + c] + Jl[r * 3 + 2] * Ad[2 * 3 + c]);
+            J2[r * 3 + c] = Jl[r * 3 + c];
+          }
+      }
+    } else {
+      const T* p1 = mp_var(g, 0, k, b);
+      const T* p2 = mp_var(g, 2, k, b);
+#pragma unroll
+      for (int i = 0; i < D; i++) pd[i] = p2[i] - p1[i];
+#pragma unroll
+      for (int i = 0; i < D * D; i++) {
+        J1[i] = (i / D == i % D) ? T(-1) : T(0);
+        J2[i] = (i / D == i % D) ? T(1) : T(0);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < D; i++) {
+      e[i] = pd[i] - dt * v1[i];
+      e[D + i] = v2[i] - v1[i];
+    }
+    if (WITH_J) {
+#pragma unroll
+      for (int r = 0; r < D; r++)
+#pragma unroll
+        for (int c = 0; c < D; c++) {
+          const bool diag = r == c;
+          T* top = S + r * stride;
+          T* bot = S + (D + r) * stride;
+          top[bp[0] + c] = J1[r * D + c];
+          top[bp[1] + c] = diag ? -dt : T(0);
+          top[bp[2] + c] = J2[r * D + c];
+          top[bp[3] + c] = T(0);
+          bot[bp[0] + c] = T(0);
+          bot[bp[1] + c] = diag ? T(-1) : T(0);
+          bot[bp[2] + c] = T(0);
+          bot[bp[3] + c] = diag ? T(1) : T(0);
+        }
+    }
+  } else if constexpr (KIND == THB_COST_HINGE) {
+    // limits tightened by the threshold; above the upper limit wins (misc.py:62-84)
+    const T* x = mp_var(g, 0, k, b);
+    const T* dl = mp_aux(g, 0, k, b);
+    const T* ul = mp_aux(g, 1, k, b);
+    const T* th = mp_aux(g, 2, k, b);
+#pragma unroll
+    for (int i = 0; i < D; i++) {
+      const T down = dl[i] + th[i], up = ul[i] - th[i], v = x[i];
+      const bool below = v < down, above = v > up;
+      e[i] = above ? (v - up) : (below ? (down - v) : T(0));
+      if (WITH_J) {
+#pragma unroll
+        for (int c = 0; c < D; c++) S[i * stride + bp[0] + c] = (c == i) ? (above ? T(1) : (below ? T(-1) : T(0))) : T(0);
+      }
+    }
+  } else {   // Nonholonomic (misc.py:126-178)
+    const T* v = mp_var(g, 1, k, b);
+    if constexpr (KIND == THB_COST_NONHOLONOMIC_SE2) {
+      e[0] = v[1];
+      if (WITH_J) {
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+          S[bp[0] + c] = T(0);
+          S[bp[1] + c] = (c == 1) ? T(1) : T(0);
+        }
+      }
+    } else {
+      const T* p = mp_var(g, 0, k, b);
+      T s, c;
+      t_sincos(p[2], &s, &c);
+      e[0] = v[1] * c - v[0] * s;
+      if (WITH_J) {
+        S[bp[0] + 0] = T(0);
+        S[bp[0] + 1] = T(0);
+        S[bp[0] + 2] = -(v[1] * s + v[0] * c);
+        S[bp[1] + 0] = -s;
+        S[bp[1] + 1] = c;
+        S[bp[1] + 2] = T(0);
+      }
+    }
+  }
+}
+
+// The cost weight of one (k, b): per-row factors (Scale / Diagonal) or the GP weight's upper factor L^T = (chol S)^T (x) (chol Qc_inv)^T,
+// S = [[12/dt^3, -6/dt^2], [-6/dt^2, 4/dt]] (double_integrator.py:131-152): L^T = [[a U, b U], [0, c U]] with U = chol(Qc_inv)^T.
+template <typename T, int DIM, int D> struct MpWeight {
+  bool gp;
+  T w[DIM];
+  T a, bq, c, U[D * D];
+
+  __device__ __forceinline__ bool load(const GroupDev<T>& g, int k, int64_t b) {
+    gp = g.weight_kind == THB_WEIGHT_GP;
+    if (!gp) return load_weight<T, DIM>(g, k, b, w);
+    const T* Q = g.w[k] + (int64_t)g.bstride[k * 4 + 3] * b;
+    const T dt = mp_aux(g, 1, k, b)[0];
+    T L[D * D];
+#pragma unroll
+    for (int j = 0; j < D; j++) {
+      T s = Q[j * D + j];
+#pragma unroll
+      for (int q = 0; q < j; q++) s -= L[j * D + q] * L[j * D + q];
+      const T ljj = t_sqrt(s);
+      L[j * D + j] = ljj;
+#pragma unroll
+      for (int i = j + 1; i < D; i++) {
+        T t = Q[i * D + j];
+#pragma unroll
+        for (int q = 0; q < j; q++) t -= L[i * D + q] * L[j * D + q];
+        L[i * D + j] = t / ljj;
+      }
+    }
+#pragma unroll
+    for (int p = 0; p < D; p++)
+#pragma unroll
+      for (int q = 0; q < D; q++) U[p * D + q] = (q >= p) ? L[q * D + p] : T(0);
+    a = t_sqrt(T(12) / (dt * dt * dt));
+    bq = (T(-6) / (dt * dt)) / a;
+    c = t_sqrt(T(4) / dt - bq * bq);
+    return false;
+  }
+  // columns 0..ncols-1 of the DIM x ld row block v (ncols = 1, ld = 1: a vector) <- W v
+  __device__ __forceinline__ void apply(T* v, int ld, int ncols) const {
+    if (!gp) {
+      for (int j = 0; j < ncols; j++)
+#pragma unroll
+        for (int r = 0; r < DIM; r++) v[r * ld + j] *= w[r];
+      return;
+    }
+    if constexpr (DIM == 2 * D) {
+      for (int j = 0; j < ncols; j++) {
+        T top[D], bot[D];
+#pragma unroll
+        for (int p = 0; p < D; p++) { top[p] = v[p * ld + j]; bot[p] = v[(D + p) * ld + j]; }
+#pragma unroll
+        for (int p = 0; p < D; p++) {
+          T st = T(0), sb = T(0);
+#pragma unroll
+          for (int q = p; q < D; q++) {
+            st += U[p * D + q] * (a * top[q] + bq * bot[q]);
+            sb += U[p * D + q] * bot[q];
+          }
+          v[p * ld + j] = st;
+          v[(D + p) * ld + j] = c * sb;
+        }
+      }
+    }
+  }
+};
+
+template <typename T, int KIND, int D>
+__global__ void __launch_bounds__(128) linearize_mp_kernel(GroupDev<T> g, int64_t B, T* __restrict__ A_val, int64_t nnz,
+                                                           T* __restrict__ bvec, int64_t m) {
+  using M = Mp<KIND, D>;
+  extern __shared__ double lin_stage_raw[];
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const bool valid = t < (int64_t)g.K * B;     // (no early exit: every lane takes part in the warp-cooperative store below)
+  const int k = valid ? (int)(t / B) : 0;
+  const int64_t b = valid ? t - (int64_t)k * B : 0;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T* stage = reinterpret_cast<T*>(lin_stage_raw) + (size_t)warp * 32 * (M::NV + 1);
+  T* mine = stage + lane * (M::NV + 1);
+  const int stride = g.a_stride[k];
+  const int nv = M::DIM * stride;              // <= NV: the row block spans the cost function's own variables
+  int bp[M::NVARS];
+#pragma unroll
+  for (int v = 0; v < M::NVARS; v++) bp[v] = g.bp[k * M::BPW + v];
+  T e[M::DIM];
+  MpWeight<T, M::DIM, D> W;
+  if (W.load(g, k, b)) {   // every weight of this (k, b) is zero: masked cost function
+#pragma unroll
+    for (int r = 0; r < M::DIM; r++) e[r] = T(0);
+    for (int i = 0; i < nv; i++) mine[i] = T(0);
+  } else {
+    mp_cost<T, KIND, D, true>(g, k, b, e, mine, stride, bp);
+    W.apply(e, 1, 1);
+    W.apply(mine, stride, stride);
+  }
+  __syncwarp();
+  const unsigned long long my_dst = valid ? reinterpret_cast<unsigned long long>(A_val + b * nnz + g.a_off[k]) : 0ull;
+  for (int i = 0; i < 32; i++) {
+    const unsigned long long d = __shfl_sync(0xffffffffu, my_dst, i);
+    const int nvi = __shfl_sync(0xffffffffu, nv, i);
+    if (d != 0ull) {
+      T* dst = reinterpret_cast<T*>(d);
+      const T* src = stage + i * (M::NV + 1);
+      for (int v = lane; v < nvi; v += 32) dst[v] = src[v];
+    }
+  }
+  if (valid) {
+    T* brow = bvec + b * m + g.row0[k];
+#pragma unroll
+    for (int r = 0; r < M::DIM; r++) brow[r] = -e[r];
+  }
+}
+
+template <typename T, int KIND, int D>
+__global__ void __launch_bounds__(128) error_mp_kernel(GroupDev<T> g, int64_t B, T* __restrict__ partial) {
+  using M = Mp<KIND, D>;
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int nchunks = (g.K + kErrCostsPerThread - 1) / kErrCostsPerThread;
+  if (t >= (int64_t)nchunks * B) return;
+  const int c = (int)(t / B);
+  const int64_t b = t - (int64_t)c * B;
+  T acc = T(0);
+  const int k1 = min(g.K, (c + 1) * kErrCostsPerThread);
+  for (int k = c * kErrCostsPerThread; k < k1; k++) {
+    MpWeight<T, M::DIM, D> W;
+    if (W.load(g, k, b)) continue;
+    T e[M::DIM];
+    mp_cost<T, KIND, D, false>(g, k, b, e, nullptr, 0, nullptr);
+    W.apply(e, 1, 1);
+    T x = T(0);
+#pragma unroll
+    for (int r = 0; r < M::DIM; r++) x += e[r] * e[r];
+    acc += x;
+  }
+  partial[(int64_t)c * B + b] = acc * T(0.5);
+}
+
+// Checks the fields the motion-planning kinds read; the pose dof D of the kernel instance (0 = no fused kernel for this group).
+static int mp_dof(const thb_cost_group* g) {
+  const bool gp = g->weight_kind == THB_WEIGHT_GP;
+  if (g->weight_kind != THB_WEIGHT_SCALE && g->weight_kind != THB_WEIGHT_DIAGONAL && !gp) return 0;
+  switch (g->kind) {
+    case THB_COST_COLLISION2D_POINT2:
+    case THB_COST_COLLISION2D_SE2:
+      if (gp || g->aux2 == nullptr || g->aux3 == nullptr || g->aux4 == nullptr || g->bstride2 == nullptr || g->grid_rows < 1 || g->grid_cols < 1)
+        return 0;
+      return g->kind == THB_COST_COLLISION2D_POINT2 ? 2 : 3;
+    case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
+    case THB_COST_DOUBLE_INTEGRATOR_SE2: {
+      if (g->x2 == nullptr || g->x3 == nullptr || g->bstride3 == nullptr || (gp && (g->aux2 == nullptr || g->bstride2 == nullptr))) return 0;
+      const int d = g->dim / 2;
+      if (g->kind == THB_COST_DOUBLE_INTEGRATOR_SE2) return g->dim == 6 ? 3 : 0;
+      return (g->dim % 2 == 0 && d >= 1 && d <= 3) ? d : 0;
+    }
+    case THB_COST_HINGE:
+      if (gp || g->aux2 == nullptr || g->aux3 == nullptr || g->bstride2 == nullptr) return 0;
+      return (g->dim >= 1 && g->dim <= 3) ? g->dim : 0;
+    case THB_COST_NONHOLONOMIC_SE2:
+    case THB_COST_NONHOLONOMIC_VECTOR: return gp ? 0 : 3;
+    default: return 0;
+  }
+}
+
 template <typename T> __global__ void error_reduce_kernel(const T* __restrict__ partial, int nchunks, int64_t B, T* __restrict__ err) {
   const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
@@ -763,6 +1112,45 @@ static int linearize_group(const thb_cost_group* g, int64_t B, T* A_val, int64_t
       if (g->aux2 == nullptr || g->aux3 == nullptr || g->aux4 == nullptr || g->bstride2 == nullptr) return THB_ERR_BAD_ARG;
       linearize_reprojection_kernel<T><<<grid, 128, 0, cs>>>(d, B, A_val, nnz, b, m);
       break;
+    case THB_COST_COLLISION2D_POINT2:
+    case THB_COST_COLLISION2D_SE2:
+    case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
+    case THB_COST_DOUBLE_INTEGRATOR_SE2:
+    case THB_COST_HINGE:
+    case THB_COST_NONHOLONOMIC_SE2:
+    case THB_COST_NONHOLONOMIC_VECTOR: {
+      const int dof = mp_dof(g);
+      if (dof == 0) return THB_ERR_BAD_ARG;
+#define THB_MP_LAUNCH(KIND, D)                                                                                                \
+  do {                                                                                                                      \
+    const size_t smem_ = (size_t)4 * 32 * (Mp<KIND, D>::NV + 1) * sizeof(T);                                                \
+    static bool attr_ = false;                                                                                              \
+    if (!attr_ && smem_ > 48 * 1024) {                                                                                      \
+      THB_CUDA(cudaFuncSetAttribute(linearize_mp_kernel<T, KIND, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_)); \
+      attr_ = true;                                                                                                         \
+    }                                                                                                                       \
+    linearize_mp_kernel<T, KIND, D><<<grid, 128, smem_, cs>>>(d, B, A_val, nnz, b, m);                                      \
+  } while (0)
+      switch (g->kind) {
+        case THB_COST_COLLISION2D_POINT2: THB_MP_LAUNCH(THB_COST_COLLISION2D_POINT2, 2); break;
+        case THB_COST_COLLISION2D_SE2: THB_MP_LAUNCH(THB_COST_COLLISION2D_SE2, 3); break;
+        case THB_COST_DOUBLE_INTEGRATOR_SE2: THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_SE2, 3); break;
+        case THB_COST_NONHOLONOMIC_SE2: THB_MP_LAUNCH(THB_COST_NONHOLONOMIC_SE2, 3); break;
+        case THB_COST_NONHOLONOMIC_VECTOR: THB_MP_LAUNCH(THB_COST_NONHOLONOMIC_VECTOR, 3); break;
+        case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
+          if (dof == 1) THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 1);
+          else if (dof == 2) THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 2);
+          else THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 3);
+          break;
+        default:   // THB_COST_HINGE
+          if (dof == 1) THB_MP_LAUNCH(THB_COST_HINGE, 1);
+          else if (dof == 2) THB_MP_LAUNCH(THB_COST_HINGE, 2);
+          else THB_MP_LAUNCH(THB_COST_HINGE, 3);
+          break;
+      }
+#undef THB_MP_LAUNCH
+      break;
+    }
     default: return THB_ERR_UNSUPPORTED;
   }
   THB_CHECK_LAUNCH();
@@ -788,6 +1176,34 @@ template <typename T> static int error_group(const thb_cost_group* g, int64_t B,
       if (g->aux2 == nullptr || g->aux3 == nullptr || g->aux4 == nullptr || g->bstride2 == nullptr) return THB_ERR_BAD_ARG;
       error_reprojection_kernel<T><<<grid, 128, 0, cs>>>(d, B, partial);
       break;
+    case THB_COST_COLLISION2D_POINT2:
+    case THB_COST_COLLISION2D_SE2:
+    case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
+    case THB_COST_DOUBLE_INTEGRATOR_SE2:
+    case THB_COST_HINGE:
+    case THB_COST_NONHOLONOMIC_SE2:
+    case THB_COST_NONHOLONOMIC_VECTOR: {
+      const int dof = mp_dof(g);
+      if (dof == 0) return THB_ERR_BAD_ARG;
+      switch (g->kind) {
+        case THB_COST_COLLISION2D_POINT2: error_mp_kernel<T, THB_COST_COLLISION2D_POINT2, 2><<<grid, 128, 0, cs>>>(d, B, partial); break;
+        case THB_COST_COLLISION2D_SE2: error_mp_kernel<T, THB_COST_COLLISION2D_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
+        case THB_COST_DOUBLE_INTEGRATOR_SE2: error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
+        case THB_COST_NONHOLONOMIC_SE2: error_mp_kernel<T, THB_COST_NONHOLONOMIC_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
+        case THB_COST_NONHOLONOMIC_VECTOR: error_mp_kernel<T, THB_COST_NONHOLONOMIC_VECTOR, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
+        case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
+          if (dof == 1) error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 1><<<grid, 128, 0, cs>>>(d, B, partial);
+          else if (dof == 2) error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 2><<<grid, 128, 0, cs>>>(d, B, partial);
+          else error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 3><<<grid, 128, 0, cs>>>(d, B, partial);
+          break;
+        default:   // THB_COST_HINGE
+          if (dof == 1) error_mp_kernel<T, THB_COST_HINGE, 1><<<grid, 128, 0, cs>>>(d, B, partial);
+          else if (dof == 2) error_mp_kernel<T, THB_COST_HINGE, 2><<<grid, 128, 0, cs>>>(d, B, partial);
+          else error_mp_kernel<T, THB_COST_HINGE, 3><<<grid, 128, 0, cs>>>(d, B, partial);
+          break;
+      }
+      break;
+    }
     default: return THB_ERR_UNSUPPORTED;
   }
   THB_CHECK_LAUNCH();

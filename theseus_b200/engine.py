@@ -33,6 +33,18 @@ def _batched_torch_route() -> bool:
     return os.environ.get("THB_BATCHED_TORCH_ROUTE", "0") == "1"
 
 
+_WEIGHT_GP = 2                                  # thb_weight_kind THB_WEIGHT_GP
+_DI_KINDS = (10, 11)                            # THB_COST_DOUBLE_INTEGRATOR_VECTOR / _SE2: the kinds that take a GP weight
+_COLLISION_KINDS = (8, 9)                       # THB_COST_COLLISION2D_POINT2 / _SE2: aux = origin, sdf data, cell size, eps
+
+
+def _grid_shape(kind, aux):
+    """(rows, cols) of a collision cost function's SDF grid (part of its group key: the kernel indexes the grids with the group's shape)."""
+    if kind in _COLLISION_KINDS:
+        return tuple(int(n) for n in aux[1].tensor.shape[-2:])
+    return (0, 0)
+
+
 def _require_cuda_device(device):
     """The product has no CPU path: fail loudly.  (tests/test_simt_engine_emulation.py replaces this guard AND the library by a host
     emulation of the kernels to exercise the host code without a GPU; nothing in the package does.)"""
@@ -92,15 +104,20 @@ class Engine:
             if kind is None or cf.weight.WEIGHT_KIND < 0:   # no fused kernel for this cost function / a user-defined CostWeight
                 self.generic.append(f)
                 continue
-            key = (kind, cf.weight.WEIGHT_KIND, cf.dim(), int(getattr(cf, "robust_kind", 0)))
+            if cf.weight.WEIGHT_KIND == _WEIGHT_GP and kind not in _DI_KINDS:   # a matrix weight the kernel of this kind does not apply
+                self.generic.append(f)
+                continue
+            key = (kind, cf.weight.WEIGHT_KIND, cf.dim(), int(getattr(cf, "robust_kind", 0)), _grid_shape(kind, self._aux_of[-1]))
             groups.setdefault(key, []).append(f)
         self.groups: List[_Group] = []
         dev = self.device
-        for (kind, wkind, dim, robust), idx in groups.items():
+        for (kind, wkind, dim, robust, grid), idx in groups.items():
             g = _Group(kind, wkind, dim, idx)
             g.robust = robust
+            g.grid = grid
+            g.nvars = len(costs[idx[0]].optim_vars)
             ii = np.array(idx, dtype=np.int64)
-            bp = np.zeros((g.K, 2), dtype=np.int32)
+            bp = np.zeros((g.K, max(2, g.nvars)), dtype=np.int32)
             for r, f in enumerate(idx):
                 p = S.block_pointers[f]
                 bp[r, : len(p)] = p
@@ -243,24 +260,34 @@ class Engine:
 
         for g in self.groups:
             x0, x1, aux, w = [], [], [], []
+            x23 = [[], []]
             extra = [[], [], []]
             n_extra = len(self._aux_of[g.cost_indices[0]]) - 1
             bs = np.zeros((g.K, 4), dtype=np.int32)
             bs2 = np.zeros((g.K, 3), dtype=np.int32)
+            bs3 = np.zeros((g.K, 2), dtype=np.int32)
             for r, f in enumerate(g.cost_indices):
                 cf = self.costs[f]
                 ov = cf.optim_vars
                 t0 = optim_tensor(ov[0])
                 t1 = optim_tensor(ov[1]) if len(ov) > 1 else t0
                 auxs = [aux_tensor(a) for a in self._aux_of[f]]
+                a0 = auxs[0] if auxs else t0          # a kind without aux tensors (Nonholonomic) never reads `aux`
                 tw = aux_tensor(cf.weight.weight_tensor())
-                x0.append(t0); x1.append(t1); aux.append(auxs[0]); w.append(tw)
-                bs[r] = (bstride(t0), bstride(t1), bstride(auxs[0]), bstride(tw))
+                x0.append(t0); x1.append(t1); aux.append(a0); w.append(tw)
+                bs[r] = (bstride(t0), bstride(t1), 0 if not auxs else bstride(a0), bstride(tw))
                 for q in range(n_extra):
                     extra[q].append(auxs[1 + q])
                     bs2[r, q] = bstride(auxs[1 + q])
+                for q in range(g.nvars - 2):
+                    t = optim_tensor(ov[2 + q])
+                    x23[q].append(t)
+                    bs3[r, q] = bstride(t)
             keep = dict(x0=self._ptr_array(x0), x1=self._ptr_array(x1), aux=self._ptr_array(aux), w=self._ptr_array(w),
-                        bstride=_dev(bs, self.device), tensors=(x0, x1, aux, w, extra))
+                        bstride=_dev(bs, self.device), tensors=(x0, x1, aux, w, extra, x23))
+            x23p = [self._ptr_array(x23[q]) if g.nvars > 2 + q else None for q in range(2)]
+            keep["x23"] = x23p
+            keep["bstride3"] = _dev(bs3, self.device)
             ex = [self._ptr_array(extra[q]) if n_extra > q else None for q in range(3)]
             keep["extra"] = ex
             keep["bstride2"] = _dev(bs2, self.device)
@@ -278,7 +305,9 @@ class Engine:
                 aux2=ex[0].data_ptr() if ex[0] is not None else None, aux3=ex[1].data_ptr() if ex[1] is not None else None,
                 aux4=ex[2].data_ptr() if ex[2] is not None else None, bstride2=keep["bstride2"].data_ptr(),
                 robust_kind=g.robust, reserved0=0, log_radius=lr_ptr.data_ptr() if lr_ptr is not None else None,
-                bstride_lr=lr_bs.data_ptr() if lr_bs is not None else None)
+                bstride_lr=lr_bs.data_ptr() if lr_bs is not None else None,
+                x2=x23p[0].data_ptr() if x23p[0] is not None else None, x3=x23p[1].data_ptr() if x23p[1] is not None else None,
+                bstride3=keep["bstride3"].data_ptr(), grid_rows=g.grid[0], grid_cols=g.grid[1])
             g.bound[which] = (st, keep)
         # NOTE: _bind may itself rebind non-contiguous tensors (bumping the counter); read it afterwards.
         self._bind_stamp[which] = Variable._global_updates
@@ -396,6 +425,7 @@ class Engine:
     def _user_costs(self, ids) -> bool:
         """True if any of these cost functions is a user-defined subclass (own error() / jacobians()): those run per cost function."""
         return any(self.costs[f]._user_defined("jacobians") or self.costs[f]._user_defined("error") or self.costs[f].weight.WEIGHT_KIND < 0
+                   or self.costs[f].weight.WEIGHT_KIND == _WEIGHT_GP
                    or getattr(getattr(self.costs[f], "cost_function", None), "_user_defined", lambda w: False)("jacobians") for f in ids)
 
     def _route(self, which: str):
