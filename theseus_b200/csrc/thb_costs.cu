@@ -448,6 +448,13 @@ __global__ void __launch_bounds__(128) error_reprojection_kernel(GroupDev<T> g, 
 }
 
 // Difference on Vector/Point: e = (x - target) * w ; J = I * w   (geometry/vector.py local/jacobians)
+// true if every weight of this (k, b) is zero: the cost function is masked like the other kinds (load_weight), its x / target not read
+template <typename T> __device__ __forceinline__ bool vector_masked(const GroupDev<T>& g, const T* wp) {
+  if (g.weight_kind == THB_WEIGHT_SCALE) return wp[0] == T(0);
+  for (int r = 0; r < g.dim; r++)
+    if (wp[r] != T(0)) return false;
+  return true;
+}
 template <typename T>
 __global__ void linearize_vector_kernel(GroupDev<T> g, int64_t B, T* __restrict__ A_val, int64_t nnz,
                                         T* __restrict__ bvec, int64_t m) {
@@ -463,10 +470,11 @@ __global__ void linearize_vector_kernel(GroupDev<T> g, int64_t B, T* __restrict_
   const int stride = g.a_stride[k];
   const int bp0 = g.bp[k * 2 + 0];
   T* brow = bvec + b * m + g.row0[k];
+  const bool masked = vector_masked(g, wp);
   for (int r = 0; r < d; r++) {
-    const T w = (g.weight_kind == THB_WEIGHT_SCALE) ? wp[0] : wp[r];
+    const T w = masked ? T(0) : ((g.weight_kind == THB_WEIGHT_SCALE) ? wp[0] : wp[r]);
     for (int c = 0; c < d; c++) Arow[r * stride + bp0 + c] = (r == c) ? w : T(0);
-    brow[r] = -((x[r] - tg[r]) * w);
+    brow[r] = masked ? T(0) : -((x[r] - tg[r]) * w);
   }
 }
 
@@ -509,6 +517,7 @@ template <typename T> __global__ void error_vector_kernel(GroupDev<T> g, int64_t
     const T* x = g.x0[k] + (int64_t)g.bstride[k * 4 + 0] * b;
     const T* tg = g.aux[k] + (int64_t)g.bstride[k * 4 + 2] * b;
     const T* wp = g.w[k] + (int64_t)g.bstride[k * 4 + 3] * b;
+    if (vector_masked(g, wp)) continue;
     for (int r = 0; r < g.dim; r++) {
       const T w = (g.weight_kind == THB_WEIGHT_SCALE) ? wp[0] : wp[r];
       const T e = (x[r] - tg[r]) * w;
