@@ -67,7 +67,14 @@ enum thb_cost_kind {
   THB_COST_HINGE = 12,
   /* Nonholonomic: x0 = pose (SE2 [B,4] / Vector [B,3]), x1 = vel [B,3]; dim 1. */
   THB_COST_NONHOLONOMIC_SE2 = 13,
-  THB_COST_NONHOLONOMIC_VECTOR = 14
+  THB_COST_NONHOLONOMIC_VECTOR = 14,
+  /* Planar pushing (theseus/embodied/motionmodel/quasi_static_pushing_planar.py:19-297): x0 = obj1, x1 = obj2, x2 = eff1, x3 = eff2
+   * (SE2 [B,4]); aux = c_square [Bc,1].  e = D V - Vp (Zhou et al. 2017), dim 3. */
+  THB_COST_QUASI_STATIC_PUSHING_PLANAR = 15,
+  /* Effector-object contact (theseus/embodied/collision/eff_obj_contact.py:21-126): x0 = obj, x1 = eff (SE2 [B,4]); aux = sdf origin
+   * [Bo,2], aux2 = sdf data [Bd,rows,cols], aux3 = cell size [Bc,1], aux4 = eff_radius [Br,1]; grid_rows / grid_cols = the grid shape.
+   * e = |sdf(R_obj^T (t_eff - t_obj)) - eff_radius|, dim 1. */
+  THB_COST_EFF_OBJ_CONTACT_PLANAR = 16
 };
 enum thb_robust_kind { THB_ROBUST_NONE = 0, THB_ROBUST_WELSCH = 1, THB_ROBUST_HUBER = 2 };
 enum thb_weight_kind {
@@ -107,13 +114,13 @@ typedef struct thb_cost_group {
   int32_t reserved0;
   const void* const* log_radius;
   const int32_t* bstride_lr;
-  /* Cost functions with more than two optimisation variables (DoubleIntegrator): device [K] pointers to the third and fourth
+  /* Cost functions with more than two optimisation variables (DoubleIntegrator, QuasiStaticPushingPlanar): device [K] pointers to the third and fourth
    * variable, their batch strides in device int32 [K,2] (NULL otherwise).  `bp` is then [K, 4]; it is [K, 2] for every kind with
    * at most two variables. */
   const void* const* x2;
   const void* const* x3;
   const int32_t* bstride3;
-  /* Collision2D: shape of the SDF grids of the group (every cost function of a group has the same one). */
+  /* Collision2D / EffectorObjectContactPlanar: shape of the SDF grids of the group (every cost function of a group has the same one). */
   int32_t grid_rows;
   int32_t grid_cols;
 } thb_cost_group;

@@ -25,6 +25,7 @@ COST_BETWEEN_SE3, COST_LOCAL_SE3, COST_BETWEEN_SO3, COST_LOCAL_SO3, COST_LOCAL_V
 COST_BETWEEN_SE2, COST_LOCAL_SE2 = 6, 7
 COST_COLLISION2D_POINT2, COST_COLLISION2D_SE2, COST_DOUBLE_INTEGRATOR_VECTOR, COST_DOUBLE_INTEGRATOR_SE2 = 8, 9, 10, 11
 COST_HINGE, COST_NONHOLONOMIC_SE2, COST_NONHOLONOMIC_VECTOR = 12, 13, 14
+COST_QUASI_STATIC_PUSHING_PLANAR, COST_EFF_OBJ_CONTACT_PLANAR = 15, 16
 WEIGHT_SCALE, WEIGHT_DIAGONAL, WEIGHT_GP = 0, 1, 2
 
 

@@ -537,12 +537,16 @@ template <typename T> __device__ __forceinline__ T t_floor(T x);
 template <> __device__ __forceinline__ float t_floor<float>(float x) { return floorf(x); }
 template <> __device__ __forceinline__ double t_floor<double>(double x) { return floor(x); }
 
+// Planar pushing (tactile pose estimation): QuasiStaticPushingPlanar (motionmodel/quasi_static_pushing_planar.py:19-297) over four SE2
+// poses and EffectorObjectContactPlanar (collision/eff_obj_contact.py:21-126) over two, both with D = 3.
 template <int KIND, int D> struct Mp {
   static constexpr bool COLL = KIND == THB_COST_COLLISION2D_POINT2 || KIND == THB_COST_COLLISION2D_SE2;
   static constexpr bool DI = KIND == THB_COST_DOUBLE_INTEGRATOR_VECTOR || KIND == THB_COST_DOUBLE_INTEGRATOR_SE2;
   static constexpr bool NH = KIND == THB_COST_NONHOLONOMIC_SE2 || KIND == THB_COST_NONHOLONOMIC_VECTOR;
-  static constexpr int DIM = (COLL || NH) ? 1 : (DI ? 2 * D : D);
-  static constexpr int NVARS = DI ? 4 : (NH ? 2 : 1);
+  static constexpr bool QSP = KIND == THB_COST_QUASI_STATIC_PUSHING_PLANAR;
+  static constexpr bool EOC = KIND == THB_COST_EFF_OBJ_CONTACT_PLANAR;
+  static constexpr int DIM = (COLL || NH || EOC) ? 1 : (DI ? 2 * D : D);
+  static constexpr int NVARS = (DI || QSP) ? 4 : ((NH || EOC) ? 2 : 1);
   static constexpr int BPW = NVARS > 2 ? NVARS : 2;   // row length of the group's bp table
   static constexpr int COLS = NVARS * D;
   static constexpr int NV = DIM * COLS;
@@ -560,35 +564,39 @@ template <typename T> __device__ __forceinline__ const T* mp_aux(const GroupDev<
   return p[k] + (int64_t)g.bstride2[k * 3 + (q - 1)] * b;
 }
 
+// Signed distance of the point (px, py) in the SDF grid data [R, C] whose cell (r, c) lies at (ox, oy) + (c, r) * cell, by bilinear
+// interpolation (signed_distance_field.py:163-241), and its gradient (jx, jy); 0 and a zero gradient outside the grid.
+template <typename T>
+__device__ __forceinline__ void sdf_lookup(const T* data, int R, int C, T ox, T oy, T cell, T px, T py, T& dist, T& jx, T& jy) {
+  const bool oob = (px < ox) || (px > ox + (T(C) - T(1)) * cell) || (py < oy) || (py > oy + (T(R) - T(1)) * cell);
+  dist = T(0), jx = T(0), jy = T(0);
+  if (!oob) {
+    const T col = (px - ox) / cell, row = (py - oy) / cell;
+    const T lr = t_floor(row), lc = t_floor(col);
+    const T hr = lr + T(1), hc = lc + T(1);
+    auto clampi = [](T v, int hi) { return !(v >= T(0)) ? 0 : (v > T(hi) ? hi : (int)v); };
+    const int lri = clampi(lr, R - 1), lci = clampi(lc, C - 1), hri = clampi(hr, R - 1), hci = clampi(hc, C - 1);
+    const T g00 = data[(int64_t)lri * C + lci], g10 = data[(int64_t)hri * C + lci];
+    const T g01 = data[(int64_t)lri * C + hci], g11 = data[(int64_t)hri * C + hci];
+    const T hrd = hr - row, hcd = hc - col, lrd = row - lr, lcd = col - lc;
+    dist = hrd * hcd * g00 + lrd * hcd * g10 + hrd * lcd * g01 + lrd * lcd * g11;
+    jx = (hrd * (g01 - g00) + lrd * (g11 - g10)) / cell;
+    jy = (hcd * (g10 - g00) + lcd * (g11 - g01)) / cell;
+  }
+}
+
 // Unweighted error e[DIM] and (WITH_J) Jacobian rows S[r * stride + bp[v] + c] of one cost function.
 template <typename T, int KIND, int D, bool WITH_J>
 __device__ __forceinline__ void mp_cost(const GroupDev<T>& g, int k, int64_t b, T* e, T* S, int stride, const int* bp) {
   using M = Mp<KIND, D>;
   if constexpr (M::COLL) {
-    // sdf by bilinear interpolation, 0 (and a zero gradient) outside the grid; e = max(eps - sdf, 0), J = -d sdf where sdf <= eps
+    // e = max(eps - sdf, 0), J = -d sdf where sdf <= eps
     const T* x = mp_var(g, 0, k, b);
-    const T px = x[0], py = x[1];
     const T* org = mp_aux(g, 0, k, b);
-    const T* data = mp_aux(g, 1, k, b);
     const T cell = mp_aux(g, 2, k, b)[0];
     const T eps = mp_aux(g, 3, k, b)[0];
-    const int R = g.grid_rows, C = g.grid_cols;
-    const T ox = org[0], oy = org[1];
-    const bool oob = (px < ox) || (px > ox + (T(C) - T(1)) * cell) || (py < oy) || (py > oy + (T(R) - T(1)) * cell);
-    T dist = T(0), jx = T(0), jy = T(0);
-    if (!oob) {
-      const T col = (px - ox) / cell, row = (py - oy) / cell;
-      const T lr = t_floor(row), lc = t_floor(col);
-      const T hr = lr + T(1), hc = lc + T(1);
-      auto clampi = [](T v, int hi) { return !(v >= T(0)) ? 0 : (v > T(hi) ? hi : (int)v); };
-      const int lri = clampi(lr, R - 1), lci = clampi(lc, C - 1), hri = clampi(hr, R - 1), hci = clampi(hc, C - 1);
-      const T g00 = data[(int64_t)lri * C + lci], g10 = data[(int64_t)hri * C + lci];
-      const T g01 = data[(int64_t)lri * C + hci], g11 = data[(int64_t)hri * C + hci];
-      const T hrd = hr - row, hcd = hc - col, lrd = row - lr, lcd = col - lc;
-      dist = hrd * hcd * g00 + lrd * hcd * g10 + hrd * lcd * g01 + lrd * lcd * g11;
-      jx = (hrd * (g01 - g00) + lrd * (g11 - g10)) / cell;
-      jy = (hcd * (g10 - g00) + lcd * (g11 - g01)) / cell;
-    }
+    T dist, jx, jy;
+    sdf_lookup(mp_aux(g, 1, k, b), g.grid_rows, g.grid_cols, org[0], org[1], cell, x[0], x[1], dist, jx, jy);
     const T err = eps - dist;
     e[0] = err < T(0) ? T(0) : err;
     if (WITH_J) {
@@ -660,6 +668,78 @@ __device__ __forceinline__ void mp_cost(const GroupDev<T>& g, int k, int64_t b, 
           bot[bp[2] + c] = T(0);
           bot[bp[3] + c] = diag ? T(1) : T(0);
         }
+    }
+  } else if constexpr (M::QSP) {
+    // p = R2^T (s2 - t2) (contact point in the frame of obj2), v = R2^T (t2 - t1), vp = R2^T (s2 - s1), w = theta(obj1^-1 obj2);
+    // e = D [v, w] - [vp, 0] with D = [[1, 0, -py], [0, 1, px], [-py, px, -c^2]]
+    const T* o1 = mp_var(g, 0, k, b);
+    const T* o2 = mp_var(g, 1, k, b);
+    const T* e1 = mp_var(g, 2, k, b);
+    const T* e2 = mp_var(g, 3, k, b);
+    const T c2 = mp_aux(g, 0, k, b)[0];
+    const T c = o2[2], s = o2[3];
+    auto unrot_x = [&](T x, T y) { return c * x + s * y; };
+    auto unrot_y = [&](T x, T y) { return -s * x + c * y; };
+    const T px = unrot_x(e2[0] - o2[0], e2[1] - o2[1]), py = unrot_y(e2[0] - o2[0], e2[1] - o2[1]);
+    const T vx = unrot_x(o2[0] - o1[0], o2[1] - o1[1]), vy = unrot_y(o2[0] - o1[0], o2[1] - o1[1]);
+    const T vpx = unrot_x(e2[0] - e1[0], e2[1] - e1[1]), vpy = unrot_y(e2[0] - e1[0], e2[1] - e1[1]);
+    const T w = t_atan2(o1[2] * s - o1[3] * c, o1[2] * c + o1[3] * s);
+    e[0] = vx - py * w - vpx;
+    e[1] = vy + px * w - vpy;
+    e[2] = -py * vx + px * vy - c2 * w;
+    if (WITH_J) {
+      // column j of variable v from the derivatives of (p, v, vp, w) along that tangent direction
+      auto col = [&](int v, int j, T dpx, T dpy, T dvx, T dvy, T dvpx, T dvpy, T dw) {
+        S[0 * stride + bp[v] + j] = dvx - w * dpy - py * dw - dvpx;
+        S[1 * stride + bp[v] + j] = dvy + w * dpx + px * dw - dvpy;
+        S[2 * stride + bp[v] + j] = -vx * dpy - py * dvx + vy * dpx + px * dvy - c2 * dw;
+      };
+      // R2^T R_x of a pose x: the rotation by x's angle minus obj2's, with columns (rc, rs) and (-rs, rc)
+      auto rel = [&](const T* x, T& rc, T& rs) { rc = c * x[2] + s * x[3]; rs = c * x[3] - s * x[2]; };
+      const T z = T(0);
+      T rc, rs;
+      rel(o1, rc, rs);   // obj1: dv/du = -R2^T R1, dw/dtheta = -1
+      col(0, 0, z, z, -rc, -rs, z, z, z);
+      col(0, 1, z, z, rs, -rc, z, z, z);
+      col(0, 2, z, z, z, z, z, z, T(-1));
+      // obj2: dp = [-I | (py, -px)], dv = [I | (vy, -vx)], dvp = [0 | (vpy, -vpx)], dw/dtheta = 1
+      col(1, 0, T(-1), z, T(1), z, z, z, z);
+      col(1, 1, z, T(-1), z, T(1), z, z, z);
+      col(1, 2, py, -px, vy, -vx, vpy, -vpx, T(1));
+      rel(e1, rc, rs);   // eff1: dvp/du = -R2^T Re1
+      col(2, 0, z, z, z, z, -rc, -rs, z);
+      col(2, 1, z, z, z, z, rs, -rc, z);
+      col(2, 2, z, z, z, z, z, z, z);
+      rel(e2, rc, rs);   // eff2: dp/du = dvp/du = R2^T Re2
+      col(3, 0, rc, rs, z, z, rc, rs, z);
+      col(3, 1, -rs, rc, z, z, -rs, rc, z);
+      col(3, 2, z, z, z, z, z, z, z);
+    }
+  } else if constexpr (M::EOC) {
+    // p = R_obj^T (t_eff - t_obj), e = |sdf(p) - r|; J = s d sdf/dp dp/d(obj, eff) with s = -1 where sdf < r (eff_obj_contact.py:101-103)
+    const T* o = mp_var(g, 0, k, b);
+    const T* ef = mp_var(g, 1, k, b);
+    const T* org = mp_aux(g, 0, k, b);
+    const T cell = mp_aux(g, 2, k, b)[0];
+    const T r = mp_aux(g, 3, k, b)[0];
+    const T c = o[2], s = o[3];
+    const T dx = ef[0] - o[0], dy = ef[1] - o[1];
+    const T px = c * dx + s * dy, py = -s * dx + c * dy;
+    T dist, jx, jy;
+    sdf_lookup(mp_aux(g, 1, k, b), g.grid_rows, g.grid_cols, org[0], org[1], cell, px, py, dist, jx, jy);
+    const T diff = dist - r;
+    e[0] = diff < T(0) ? -diff : diff;
+    if (WITH_J) {
+      const T sg = dist < r ? T(-1) : T(1);
+      const T gx = sg * jx, gy = sg * jy;
+      // dp/d obj = [[-1, 0, py], [0, -1, -px]];  dp/d eff = [R_obj^T R_eff | 0]
+      S[bp[0] + 0] = -gx;
+      S[bp[0] + 1] = -gy;
+      S[bp[0] + 2] = gx * py - gy * px;
+      const T rc = c * ef[2] + s * ef[3], rs = c * ef[3] - s * ef[2];
+      S[bp[1] + 0] = gx * rc + gy * rs;
+      S[bp[1] + 1] = -gx * rs + gy * rc;
+      S[bp[1] + 2] = T(0);
     }
   } else if constexpr (KIND == THB_COST_HINGE) {
     // limits tightened by the threshold; above the upper limit wins (misc.py:62-84)
@@ -863,6 +943,14 @@ static int mp_dof(const thb_cost_group* g) {
       return (g->dim >= 1 && g->dim <= 3) ? g->dim : 0;
     case THB_COST_NONHOLONOMIC_SE2:
     case THB_COST_NONHOLONOMIC_VECTOR: return gp ? 0 : 3;
+    case THB_COST_QUASI_STATIC_PUSHING_PLANAR:
+      if (gp || g->x2 == nullptr || g->x3 == nullptr || g->bstride3 == nullptr || g->dim != 3) return 0;
+      return 3;
+    case THB_COST_EFF_OBJ_CONTACT_PLANAR:
+      if (gp || g->aux2 == nullptr || g->aux3 == nullptr || g->aux4 == nullptr || g->bstride2 == nullptr || g->grid_rows < 1 || g->grid_cols < 1 ||
+          g->dim != 1)
+        return 0;
+      return 3;
     default: return 0;
   }
 }
@@ -1127,7 +1215,9 @@ static int linearize_group(const thb_cost_group* g, int64_t B, T* A_val, int64_t
     case THB_COST_DOUBLE_INTEGRATOR_SE2:
     case THB_COST_HINGE:
     case THB_COST_NONHOLONOMIC_SE2:
-    case THB_COST_NONHOLONOMIC_VECTOR: {
+    case THB_COST_NONHOLONOMIC_VECTOR:
+    case THB_COST_QUASI_STATIC_PUSHING_PLANAR:
+    case THB_COST_EFF_OBJ_CONTACT_PLANAR: {
       const int dof = mp_dof(g);
       if (dof == 0) return THB_ERR_BAD_ARG;
 #define THB_MP_LAUNCH(KIND, D)                                                                                                \
@@ -1146,6 +1236,8 @@ static int linearize_group(const thb_cost_group* g, int64_t B, T* A_val, int64_t
         case THB_COST_DOUBLE_INTEGRATOR_SE2: THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_SE2, 3); break;
         case THB_COST_NONHOLONOMIC_SE2: THB_MP_LAUNCH(THB_COST_NONHOLONOMIC_SE2, 3); break;
         case THB_COST_NONHOLONOMIC_VECTOR: THB_MP_LAUNCH(THB_COST_NONHOLONOMIC_VECTOR, 3); break;
+        case THB_COST_QUASI_STATIC_PUSHING_PLANAR: THB_MP_LAUNCH(THB_COST_QUASI_STATIC_PUSHING_PLANAR, 3); break;
+        case THB_COST_EFF_OBJ_CONTACT_PLANAR: THB_MP_LAUNCH(THB_COST_EFF_OBJ_CONTACT_PLANAR, 3); break;
         case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
           if (dof == 1) THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 1);
           else if (dof == 2) THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 2);
@@ -1191,7 +1283,9 @@ template <typename T> static int error_group(const thb_cost_group* g, int64_t B,
     case THB_COST_DOUBLE_INTEGRATOR_SE2:
     case THB_COST_HINGE:
     case THB_COST_NONHOLONOMIC_SE2:
-    case THB_COST_NONHOLONOMIC_VECTOR: {
+    case THB_COST_NONHOLONOMIC_VECTOR:
+    case THB_COST_QUASI_STATIC_PUSHING_PLANAR:
+    case THB_COST_EFF_OBJ_CONTACT_PLANAR: {
       const int dof = mp_dof(g);
       if (dof == 0) return THB_ERR_BAD_ARG;
       switch (g->kind) {
@@ -1200,6 +1294,10 @@ template <typename T> static int error_group(const thb_cost_group* g, int64_t B,
         case THB_COST_DOUBLE_INTEGRATOR_SE2: error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
         case THB_COST_NONHOLONOMIC_SE2: error_mp_kernel<T, THB_COST_NONHOLONOMIC_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
         case THB_COST_NONHOLONOMIC_VECTOR: error_mp_kernel<T, THB_COST_NONHOLONOMIC_VECTOR, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
+        case THB_COST_QUASI_STATIC_PUSHING_PLANAR:
+          error_mp_kernel<T, THB_COST_QUASI_STATIC_PUSHING_PLANAR, 3><<<grid, 128, 0, cs>>>(d, B, partial);
+          break;
+        case THB_COST_EFF_OBJ_CONTACT_PLANAR: error_mp_kernel<T, THB_COST_EFF_OBJ_CONTACT_PLANAR, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
         case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
           if (dof == 1) error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 1><<<grid, 128, 0, cs>>>(d, B, partial);
           else if (dof == 2) error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 2><<<grid, 128, 0, cs>>>(d, B, partial);

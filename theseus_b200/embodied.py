@@ -1,19 +1,21 @@
-"""`th.eb` namespace of the reference (theseus/embodied/__init__.py): Between / Local / Reprojection have fused CUDA schemas;
-MovingFrameBetween runs on the torch path (torch.func Jacobians + tangent-space projection, like an AutoDiffCostFunction)."""
+"""`th.eb` namespace of the reference (theseus/embodied/__init__.py): Between / Local / Reprojection, the planar-pushing and the
+motion-planning cost functions have fused CUDA schemas; MovingFrameBetween runs on the torch path (torch.func Jacobians + tangent-space
+projection, like an AutoDiffCostFunction)."""
 from typing import List, Optional, Tuple, Union
 
 import torch
 
 from .core import Between, CostFunction, CostWeight, Difference, Local, Reprojection  # noqa: F401
-from .core import (COST_COLLISION2D_POINT2, COST_COLLISION2D_SE2, COST_DOUBLE_INTEGRATOR_SE2, COST_DOUBLE_INTEGRATOR_VECTOR, COST_HINGE,
-                   COST_NONHOLONOMIC_SE2, COST_NONHOLONOMIC_VECTOR, WEIGHT_GP)
+from .core import (COST_COLLISION2D_POINT2, COST_COLLISION2D_SE2, COST_DOUBLE_INTEGRATOR_SE2, COST_DOUBLE_INTEGRATOR_VECTOR,
+                   COST_EFF_OBJ_CONTACT_PLANAR, COST_HINGE, COST_NONHOLONOMIC_SE2, COST_NONHOLONOMIC_VECTOR, COST_QUASI_STATIC_PUSHING_PLANAR,
+                   WEIGHT_GP)
 from .geometry import SE2, LieGroup, Point2, Point3, Variable, Vector, as_variable
 
 
 class MovingFrameBetween(CostFunction):
     """theseus/embodied/measurements/moving_frame_between.py:14-77:
         e = log(Z^-1 ((F1^-1 P1)^-1 (F2^-1 P2)))        optim vars: frame1, frame2, pose1, pose2 (SE2 or SE3); aux: measurement.
-    No fused kernel (the engine's schemas hold at most two variables): torch path.  NOTE the reference's Jacobians are those of the
+    No fused kernel: torch path.  NOTE the reference's Jacobians are those of the
     group-valued D = (F1^-1 P1)^-1 (F2^-1 P2) in ITS tangent space (moving_frame_between.py:46-65 chains the `between` Jacobians and
     stops there) -- the d log factor of the final `measurement.local(D)` is not applied.  For drop-in parity the same quantity is
     computed here: Euclidean torch.func Jacobian of D, input side projected like every AutoDiff Jacobian, output side converted from a
@@ -82,7 +84,8 @@ class QuasiStaticPushingPlanar(CostFunction):
     al. 2017): object poses obj1, obj2 and end-effector poses eff1, eff2 (SE2) at consecutive times, aux c_square;
         e = D V - Vp,  V = [R2^T (t_o2 - t_o1), theta(o1^-1 o2)],  Vp = [R2^T (t_e2 - t_e1), 0],
         D = [[1, 0, -py], [0, 1, px], [-py, px, -c^2]],  (px, py) = R2^T (t_e2 - t_o2).
-    Torch path (torch.func Jacobians + tangent-space projection = the reference's chained analytic Jacobians)."""
+    Fused kernel (THB_COST_QUASI_STATIC_PUSHING_PLANAR) when all four poses are SE2; `_torch_error` is the same error for the torch route
+    (torch.func Jacobians + tangent-space projection = the reference's chained analytic Jacobians) and the autograd tape."""
 
     def __init__(self, obj1, obj2, eff1, eff2, c_square, cost_weight: CostWeight, name: Optional[str] = None):
         from .geometry import Variable, as_variable
@@ -122,6 +125,8 @@ class QuasiStaticPushingPlanar(CostFunction):
         return torch.stack((ex, ey, et), dim=-1)
 
     def schema(self):
+        if all(isinstance(v, SE2) for v in (self.obj1, self.obj2, self.eff1, self.eff2)):
+            return COST_QUASI_STATIC_PUSHING_PLANAR, [self.c_square]
         return None, []
 
 
@@ -129,8 +134,9 @@ class EffectorObjectContactPlanar(CostFunction):
     """theseus/embodied/collision/eff_obj_contact.py:21-126 (+ SignedDistanceField2D.signed_distance, collision/signed_distance_field.py:
     163-241): the end effector (a disc of radius eff_radius at eff.xy) touches the object whose signed distance field is given in the
     object frame:  e = | sdf(R_obj^T (t_eff - t_obj)) - eff_radius |,  dim 1.  sdf = bilinear interpolation of sdf_data [Bs, rows, cols]
-    (cell (r,c) at origin + (c, r) * cell_size), 0 outside the grid.  Torch path; autograd of the bilinear form is exactly the
-    reference's analytic gradient, the sign flip for dist < radius is d|.|."""
+    (cell (r,c) at origin + (c, r) * cell_size), 0 outside the grid.  Fused kernel (THB_COST_EFF_OBJ_CONTACT_PLANAR) when obj and eff
+    are SE2, with the reference's Jacobian sign (-1 where dist < radius, +1 otherwise).  `_torch_error` serves the torch route and the
+    autograd tape: autograd of the bilinear form is exactly the reference's analytic gradient, the sign flip is d|.| (0 at dist == radius)."""
 
     def __init__(self, obj, eff, sdf_origin, sdf_data, sdf_cell_size, eff_radius, cost_weight: CostWeight, name: Optional[str] = None,
                  use_huber_loss: bool = False):
@@ -170,6 +176,8 @@ class EffectorObjectContactPlanar(CostFunction):
         return (dist - radius).abs().unsqueeze(-1)
 
     def schema(self):
+        if isinstance(self.obj, SE2) and isinstance(self.eff, SE2):
+            return COST_EFF_OBJ_CONTACT_PLANAR, [self.sdf_origin, self.sdf_data, self.sdf_cell_size, self.eff_radius]
         return None, []
 
 

@@ -35,12 +35,12 @@ def _batched_torch_route() -> bool:
 
 _WEIGHT_GP = 2                                  # thb_weight_kind THB_WEIGHT_GP
 _DI_KINDS = (10, 11)                            # THB_COST_DOUBLE_INTEGRATOR_VECTOR / _SE2: the kinds that take a GP weight
-_COLLISION_KINDS = (8, 9)                       # THB_COST_COLLISION2D_POINT2 / _SE2: aux = origin, sdf data, cell size, eps
+_SDF_KINDS = (8, 9, 16)                         # THB_COST_COLLISION2D_POINT2 / _SE2, THB_COST_EFF_OBJ_CONTACT_PLANAR: aux2 = the sdf data
 
 
 def _grid_shape(kind, aux):
-    """(rows, cols) of a collision cost function's SDF grid (part of its group key: the kernel indexes the grids with the group's shape)."""
-    if kind in _COLLISION_KINDS:
+    """(rows, cols) of an SDF cost function's grid (part of its group key: the kernel indexes the grids with the group's shape)."""
+    if kind in _SDF_KINDS:
         return tuple(int(n) for n in aux[1].tensor.shape[-2:])
     return (0, 0)
 
