@@ -266,37 +266,80 @@ struct FrontRowsPanel {
   }
 };
 
-// CTA: u <- L^-1 u over the w pivot columns of a front of r rows, 32 columns at a time (u[i] at u[i * us]): a one-warp
-// triangular solve on the chunk's diagonal block, then one row per thread for the rows below it.  The border part of u ends as
-// u_b - P y.  Both the substitution kernel and the fused factor kernel run this same code (each row's sum in the same order whichever
-// thread owns it), so their y and border vectors are bitwise equal.
-template <int THREADS, typename Rows>
+// Barrier over the GROUP threads that run front_forward_elim: the whole CTA, or -- a group of warps that works beside the rest of the
+// CTA -- named barrier 1 (the host emulation has no named barriers and only runs the whole-CTA form)
+template <int GROUP, bool WHOLE_CTA>
+__device__ __forceinline__ void front_group_sync() {
+#ifdef THB_SIMT_EMU
+  static_assert(WHOLE_CTA, "the host emulation has no named barriers");
+  __syncthreads();
+#else
+  if constexpr (WHOLE_CTA) __syncthreads();
+  else asm volatile("bar.sync 1, %0;" ::"n"(GROUP) : "memory");
+#endif
+}
+
+// GROUP threads (tid = 0 .. GROUP - 1: a whole CTA, or its first GROUP / 32 warps): u <- L^-1 u over the w pivot columns of a front of r
+// rows, 32 columns at a time (u[i] at u[i * us]): a one-warp triangular solve on the chunk's diagonal block, then one row per thread for
+// the rows below it.  The border part of u ends as u_b - P y.  Both the substitution kernel and the fused factor kernel run this same
+// code (each row's sum in the same order, k ascending, whichever thread owns it), so their y and border vectors are bitwise equal.
+template <int GROUP, bool WHOLE_CTA, typename Rows>
 __device__ __forceinline__ void front_forward_elim(const Rows& R, double* u, int us, int w, int r, int tid, int lane) {
   for (int k0 = 0; k0 < w; k0 += 32) {
     const int cw = min(32, w - k0);
     int ld;
-    const double* T = R.diag(k0, cw, tid, THREADS, &ld);
-    __syncthreads();
+    const double* T = R.diag(k0, cw, tid, GROUP, &ld);
+    front_group_sync<GROUP, WHOLE_CTA>();
     if (tid < 32) {
       const double ui = front_warp_trsv_lower(T, ld, lane < cw ? u[(k0 + lane) * us] : 0.0, cw, lane);
       if (lane < cw) u[(k0 + lane) * us] = ui;
     }
-    __syncthreads();
+    front_group_sync<GROUP, WHOLE_CTA>();
     // rows below the chunk, one row per thread (from global memory: its 32 consecutive doubles are two cache lines, read once from DRAM)
-    for (int i = k0 + cw + tid; i < r; i += THREADS) {
+    for (int i = k0 + cw + tid; i < r; i += GROUP) {
       const double* row = R.row(i) + k0;
       double s = 0.0;
       if constexpr (Rows::kInPanel) {
+        // consecutive lanes own consecutive panel rows, whose stride is 4 mod 16 doubles: at equal k, lanes l, l + 4, l + 8, l + 12 of a
+        // half-warp would hit the same banks.  Each of them runs its (unchanged, k ascending) sum one step later than the previous one.
+        const int skew = (lane >> 2) & 3;
 #pragma unroll 2   // the factor kernel's 64 registers: a deeper unroll spills
-        for (int k = 0; k < cw; k++) s += row[k] * u[(k0 + k) * us];
+        for (int kk = 0; kk < cw + 3; kk++) {
+          const int k = kk - skew;
+          if ((unsigned)k < (unsigned)cw) s += row[k] * u[(k0 + k) * us];
+        }
       } else {
         for (int k = 0; k < cw; k++) s += row[k] * u[(k0 + k) * us];
       }
       u[i * us] -= s;
     }
-    __syncthreads();
+    front_group_sync<GROUP, WHOLE_CTA>();
   }
 }
+
+// Threads tid = 0 .. nthreads - 1: the factored panel (zeros above the diagonal of the pivot block) goes to the factor storage
+__device__ __forceinline__ void front_store_panel(double* __restrict__ Lg, const double* __restrict__ PN, int ldp, int w, int w8, int r, int tid,
+                                                  int nthreads) {
+  int i = tid / w, j = tid - i * w;
+  const int di = nthreads / w, dj = nthreads - di * w;
+  for (int e = tid; e < r * w; e += nthreads) {
+    Lg[e] = (j > i) ? 0.0 : PN[(i < w ? i : i + (w8 - w)) * ldp + j];
+    i += di; j += dj;
+    if (j >= w) { j -= w; i++; }
+  }
+}
+
+// Threads tid = 0 .. nthreads - 1, after front_forward_elim on u = U[i * ldp]: y of the pivots -> work, the border vector -> the parent
+__device__ __forceinline__ void front_store_forward(const FrontArgs& a, const double* U, int ldp, int64_t item, int t, int f_first, int w, int b,
+                                                    int tid, int nthreads) {
+  for (int i = tid; i < w; i += nthreads) a.work[item * a.p.n + f_first + i] = U[i * ldp];
+  double* ub = a.v_cur + item * a.p.varena_size + a.p.f_u_off[t];
+  for (int i = tid; i < b; i += nthreads) ub[i] = U[(w + i) * ldp];
+}
+
+// Warps of a front_small_kernel CTA that run the forward substitution while the others write the panel and form update-matrix tiles:
+// four, or half the CTA in the 64- and 128-thread instances
+__host__ __device__ constexpr int front_elim_warps(int threads) { return threads >= 256 ? 4 : threads / 64; }
 
 // Registers are capped at 64 per thread (1 024 threads per SM): the kernel is bound by the latency chain of a CTA, so resident warps count.
 template <int THREADS>
@@ -314,8 +357,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
   const int t = (int)FD[0];
   const int w = (int)FD[1], b = (int)FD[2], r = w + b;
   const int f_first = (int)FD[3];
-  const int64_t f_panel_off = FD[4], f_cb_off = FD[5];
-  const int f_cb_ld = (int)FD[6];
+  const int64_t f_panel_off = FD[4];
   const int c_begin = (int)(FD[7] & 0xffffffffLL);
   const int nch = min((int)(FD[7] >> 32), FRONT_MAX_CHILDREN);
   const int b16 = (b + 15) & ~15, w8 = (w + 7) & ~7;
@@ -342,6 +384,8 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
     (void)cbc;
   }
   for (int e = tid; e < prow * ldp; e += THREADS) sm[e] = 0.0;
+  int* next_tile = reinterpret_cast<int*>(Wd + 8);   // update-matrix tile counter, in a column of Wd's row padding that nothing else uses
+  if (tid == 0) *next_tile = 0;
   THB_PDL_WAIT();   // everything above reads the plan only; below: the children's update matrices, AtA, and every global write
 #ifndef THB_SIMT_EMU
   // forward substitution: the right-hand side of the pivots (through the permutation) and the children's border vectors are read once
@@ -434,33 +478,41 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
     for (int q = warp; q < npair; q += NW) front_tile_column<true>(PN, ldp, jb, jb + 1 + 2 * q, Wd, lane);
     __syncthreads();
   }
-  // ---- write the factored panel (zeros above the diagonal of the pivot block) ----
-  {
-    int i = tid / w, j = tid - i * w;
-    const int di = THREADS / w, dj = THREADS - di * w;
-    for (int e = tid; e < r * w; e += THREADS) {
-      Lg[e] = (j > i) ? 0.0 : PN[(i < w ? i : i + (w8 - w)) * ldp + j];
-      i += di; j += dj;
-      if (j >= w) { j -= w; i++; }
-    }
-  }
-  // ---- forward substitution on the factored panel, still in shared memory: y -> work, the border vector -> the parent ----
+  // ---- three consumers of the factored panel that share no data: the panel's copy to the factor storage (reads columns < w), the
+  // forward substitution (reads the panel, owns column w8) and the update-matrix tiles (read the border rows, columns < w8).  In a
+  // solve the first NE warps run the substitution behind their own barrier while the others write the panel and start on the tiles;
+  // they join the tile loop when they are done.  Every tile is computed the same way whichever warp takes it. ----
+#ifdef THB_SIMT_EMU   // no named barriers on the host emulation: the same three phases, each by the whole CTA, one after the other
+  front_store_panel(Lg, PN, ldp, w, w8, r, tid, THREADS);
   if (a.rhs != nullptr) {
-    front_forward_elim<THREADS>(FrontRowsPanel{PN, ldp, w, w8 - w}, U, ldp, w, r, tid, lane);
-    for (int i = tid; i < w; i += THREADS) a.work[item * p.n + f_first + i] = U[i * ldp];
-    double* ub = a.v_cur + item * p.varena_size + p.f_u_off[t];
-    for (int i = tid; i < b; i += THREADS) ub[i] = U[(w + i) * ldp];
+    front_forward_elim<THREADS, true>(FrontRowsPanel{PN, ldp, w, w8 - w}, U, ldp, w, r, tid, lane);
+    front_store_forward(a, U, ldp, item, t, f_first, w, b, tid, THREADS);
   }
+#else
+  constexpr int NE = front_elim_warps(THREADS);
+  if (a.rhs != nullptr && warp < NE) {
+    front_forward_elim<32 * NE, false>(FrontRowsPanel{PN, ldp, w, w8 - w}, U, ldp, w, r, tid, lane);
+    front_store_forward(a, U, ldp, item, t, f_first, w, b, tid, 32 * NE);
+  } else {
+    const int t0 = a.rhs != nullptr ? 32 * NE : 0;
+    front_store_panel(Lg, PN, ldp, w, w8, r, tid - t0, THREADS - t0);
+  }
+#endif
   if (b == 0) return;
-  // ---- update matrix: per 16 x 16 tile of the lower triangle  C = gathered children - P_I P_J^T, written once from registers ----
-  double* dst = a.arena_cur + item * p.arena_size + f_cb_off;
-  const int ldg_out = f_cb_ld;
+  // ---- update matrix: per 16 x 16 tile of the lower triangle  C = gathered children - P_I P_J^T, written once from registers; a warp
+  // takes its next tile from a counter in shared memory, so the warps that come late from the substitution take fewer ----
+  double* dst = a.arena_cur + item * p.arena_size + FD[5];   // (cb_off, cb_ld) are read here, not with the rest of the record: held in
+  const int ldg_out = (int)FD[6];                            // registers across the phases above they spill
   const double* P = PN + w8 * ldp;
-  const int nmt = b16 / 16, ntl = nmt * (nmt + 1) / 2;
-  for (int q = warp; q < ntl; q += NW) {
-    int R = (int)((sqrtf(8.0f * (float)q + 1.0f) - 1.0f) * 0.5f);
+  const int nmt = b16 / 16;
+  for (;;) {
+    int q = 0;
+    if (lane == 0) q = atomicAdd(next_tile, 1);
+    q = __shfl_sync(0xffffffffu, q, 0);
+    int R = (int)((sqrtf(8.0f * (float)q + 1.0f) - 1.0f) * 0.5f);   // tile q = (row R, column ct) of the lower triangle, row by row
     while ((R + 1) * (R + 2) / 2 <= q) R++;
     while (R * (R + 1) / 2 > q) R--;
+    if (R >= nmt) break;
     const int ct = q - R * (R + 1) / 2;
     // gathered children first: their loads are in flight while the tensor pipe works on -P_I P_J^T
     double gch[2][2][2] = {{{0.0, 0.0}, {0.0, 0.0}}, {{0.0, 0.0}, {0.0, 0.0}}};
@@ -737,7 +789,7 @@ __global__ void __launch_bounds__(THREADS) front_forward_kernel(FrontSolveArgs a
     }
   }
   __syncthreads();
-  front_forward_elim<THREADS>(FrontRowsGlobal{Lg, w, T}, u, 1, w, r, tid, lane);
+  front_forward_elim<THREADS, true>(FrontRowsGlobal{Lg, w, T}, u, 1, w, r, tid, lane);
   for (int i = tid; i < w; i += THREADS) a.work[item * p.n + first + i] = u[i];
   if (b > 0) {
     double* ub = a.v_cur + item * p.varena_size + p.f_u_off[t];
