@@ -25,6 +25,18 @@
 
 namespace thb {
 
+// *info <- the smallest failing position recorded so far (pos > 0; 0 = none yet).  Columns factored concurrently may fail in any order;
+// the smallest failing position is the leading minor that torch.linalg.cholesky / LAPACK potrf name, whichever thread gets there first.
+// (Defined in each kernel file rather than in thb_common.cuh: the host emulation of the kernels compiles the sources without that header.)
+__device__ __forceinline__ void record_first_failure(int* info, int pos) {
+  int old = 0;
+  while (true) {
+    const int prev = atomicCAS(info, old, pos);
+    if (prev == old || (prev != 0 && prev <= pos)) return;
+    old = prev;
+  }
+}
+
 constexpr int TM = 128;        // tile rows
 constexpr int TN = 64;         // tile cols = block-column width
 #ifndef THB_CHOL_KB
@@ -465,7 +477,7 @@ __global__ void __launch_bounds__(CHOL_THREADS, 2) chol_col_kernel(CholArgs p) {
   if (is_diag) {
     // ---------------- phase C: blocked potrf + triangular inverse of the 64x64 diagonal block ----------------
     const int fail = diag64_factor_invert(Cs + roff * SC, smem + TM * SC, Lb + ((int64_t)j * TN) * np + (int64_t)j * TN, np, Wj);
-    if (tid == 0 && fail != 0) atomicCAS(p.info + b, 0, p.info_base + j * TN + fail);
+    if (tid == 0 && fail != 0) record_first_failure(p.info + b, p.info_base + j * TN + fail);
     __threadfence();
     __syncthreads();
     if (tid == 0) {

@@ -23,6 +23,18 @@
 
 namespace thb {
 
+// *info <- the smallest failing position recorded so far (pos > 0; 0 = none yet).  Columns factored concurrently may fail in any order;
+// the smallest failing position is the leading minor that torch.linalg.cholesky / LAPACK potrf name, whichever thread gets there first.
+// (Defined in each kernel file rather than in thb_common.cuh: the host emulation of the kernels compiles the sources without that header.)
+__device__ __forceinline__ void record_first_failure(int* info, int pos) {
+  int old = 0;
+  while (true) {
+    const int prev = atomicCAS(info, old, pos);
+    if (prev == old || (prev != 0 && prev <= pos)) return;
+    old = prev;
+  }
+}
+
 // Programmatic dependent launch (sm_90+): a kernel launched with the attribute may start while its predecessor in the stream drains;
 // its CTAs run their prologue (plan descriptors, inverse maps, zero fill -- nothing the predecessor writes) and then wait for the
 // predecessor's completion (griddepcontrol.wait, which also orders its memory) before the first dependent read or any global write.
@@ -189,7 +201,7 @@ __device__ __forceinline__ void front_diag_block(double* PN, int ldp, int jb, do
   d[1] -= c1;
   __syncwarp();
   const int fail = front_leaf8(PN + (8 * jb) * ldp + 8 * jb, ldp, Wd, lane);
-  if (lane == 0 && fail != 0 && 8 * jb + fail <= w) atomicCAS(info, 0, first + 8 * jb + fail);
+  if (lane == 0 && fail != 0 && 8 * jb + fail <= w) record_first_failure(info, first + 8 * jb + fail);
 }
 
 // Warp: block column jb of the row tiles rt0 (and rt0 + 1 when TWO):  X = A - sum_k L_tile,k L_jb,k^T,  L = X W_jb^T, in place.

@@ -17,6 +17,18 @@
 
 namespace thb {
 
+// *info <- the smallest failing position recorded so far (pos > 0; 0 = none yet).  Columns factored concurrently may fail in any order;
+// the smallest failing position is the leading minor that torch.linalg.cholesky / LAPACK potrf name, whichever thread gets there first.
+// (Defined in each kernel file rather than in thb_common.cuh: the host emulation of the kernels compiles the sources without that header.)
+__device__ __forceinline__ void record_first_failure(int* info, int pos) {
+  int old = 0;
+  while (true) {
+    const int prev = atomicCAS(info, old, pos);
+    if (prev == old || (prev != 0 && prev <= pos)) return;
+    old = prev;
+  }
+}
+
 constexpr int SP_MAXD = 16;
 constexpr int SP_THREADS = 512;
 
@@ -156,7 +168,7 @@ __global__ void __launch_bounds__(SP_THREADS) sparse_factor_kernel(thb_sparse_pl
       if (d == 6) fail = potrf_inv_small<6>(D, Wj, 6);
       else if (d == 3) fail = potrf_inv_small<3>(D, Wj, 3);
       else fail = potrf_inv_small<0>(D, Wj, d);
-      if (fail != 0) atomicCAS(&s_fail, 0, p.pstart[p.f_col[e]] + fail);
+      if (fail != 0) record_first_failure(&s_fail, (int)(p.pstart[p.f_col[e]] + fail));
     }
     __syncthreads();
     // ---- T: L_ij[r,:] = U_ij[r,:] W_j^T ----

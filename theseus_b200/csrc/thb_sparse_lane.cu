@@ -24,6 +24,18 @@
 
 namespace thb {
 
+// *info <- the smallest failing position recorded so far (pos > 0; 0 = none yet).  Columns factored concurrently may fail in any order;
+// the smallest failing position is the leading minor that torch.linalg.cholesky / LAPACK potrf name, whichever thread gets there first.
+// (Defined in each kernel file rather than in thb_common.cuh: the host emulation of the kernels compiles the sources without that header.)
+__device__ __forceinline__ void record_first_failure(int* info, int pos) {
+  int old = 0;
+  while (true) {
+    const int prev = atomicCAS(info, old, pos);
+    if (prev == old || (prev != 0 && prev <= pos)) return;
+    old = prev;
+  }
+}
+
 constexpr int LN_WARPS = 4;  // warps per CTA; one warp = 32 batch lanes of one work item
 
 // Compile-time fence: every element of x must be in a register here, i.e. all the loads that produce x are issued before any
@@ -270,7 +282,7 @@ __global__ void __launch_bounds__(32 * LN_WARPS) lane_trsm_kernel(LaneArgs p, do
       for (int r = 0; r < DJ; r++)
 #pragma unroll
         for (int c = 0; c < DJ; c++) Dl[(r * DJ + c) * p.Bp] = (c < r) ? d[r * DJ + c] : (c == r ? inv[c] : 0.0);
-      if (fail != 0) atomicCAS(info + b, 0, p.t_pstart[item] + fail);
+      if (fail != 0) record_first_failure(info + b, (int)(p.t_pstart[item] + fail));
     }
     return;
   }

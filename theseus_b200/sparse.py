@@ -326,6 +326,7 @@ def _chains(N, struct, parent):
 
 
 LANE_DIMS = (1, 2, 3, 6)   # block sizes the batch-lane kernels are instantiated for (thb_sparse_lane.cu)
+ITEM_MAX_DIM = 16          # largest block size of the one-CTA-per-item kernels (SP_MAXD, thb_sparse.cu)
 LANE_HEAVY = 8             # update pairs per target block from which the split-K variant of the update kernel is used
 LN_U, LN_T, LN_S, LN_UH, LN_TU = 0, 1, 2, 3, 4
 TILE_DIM, TILE_ROWS, TILE_COLS = 6, 4, 4   # the tiled update kernel is instantiated for 6x6 blocks in 4 x 4 tiles (thb_sparse_lane.cu)

@@ -18,7 +18,7 @@ from .autograd import LinearSolveFunction, wants_grad
 from .core import Objective
 from .optimizer import (Linearization, LinearSolver, SparseLinearization, convert_to_alpha_beta_damping_tensors)
 from .frontal import build_front_plan
-from .sparse import LANE_DIMS, analyze, gram_out_offsets, piece_solve_lists, root_lane_lists, root_split, tile_lane_lists
+from .sparse import ITEM_MAX_DIM, LANE_DIMS, analyze, gram_out_offsets, piece_solve_lists, root_lane_lists, root_split, tile_lane_lists
 from .structure import ata_block_structure, build_gram_plan
 
 
@@ -103,8 +103,10 @@ class BaspachoSparseSolver(LinearSolver):
         """'lane' (batch-interleaved factor, one warp = 32 batch items, thb_sparse_lane.cu) or 'item' (one CTA per batch item,
         thb_sparse.cu).  Default: lane whenever a warp can be filled and every block size is one the lane kernels are built for."""
         if self._layout is None:
-            # default: the multifrontal layout for batches that fill the GPU (any block sizes); one CTA per item for small batches
-            self._layout = os.environ.get("THB_SPARSE_LAYOUT") or ("front" if B >= 32 else "item")
+            # default: the multifrontal layout for batches that fill the GPU and for blocks larger than the one-CTA-per-item kernels take
+            # (it takes any block size); one CTA per item for the other small batches
+            big = int(np.max(self.param_size, initial=0)) > ITEM_MAX_DIM
+            self._layout = os.environ.get("THB_SPARSE_LAYOUT") or ("front" if B >= 32 or big else "item")
             self.reset()
         if self._layout == "front":
             return "front"
@@ -114,6 +116,8 @@ class BaspachoSparseSolver(LinearSolver):
                 raise ValueError(f"layout must be 'lane', 'item', 'lane_root', 'lane_tiled' or 'lane_tiled_root', got {self._layout}")
             if self._layout != "item" and not lane_ok:
                 raise ValueError(f"layout='{self._layout}' needs block sizes in {LANE_DIMS}")
+            if self._layout == "item" and int(self._plan.dims.max(initial=0)) > ITEM_MAX_DIM:
+                raise ValueError(f"layout='item' needs block sizes <= {ITEM_MAX_DIM} (layout='front' takes any block size)")
             if self._layout in _ROOT_LAYOUTS and self._root_split() is None:
                 raise ValueError(f"layout='{self._layout}': this structure has no dense root (top chain too short)")
             return self._layout
