@@ -113,6 +113,22 @@ __device__ __forceinline__ double front_panel_in(const FrontArgs& a, const doubl
   return m >= 0 ? a.ata[item * a.ata_stride + m] : 0.0;
 }
 
+// Load through the global read-only path.  The gathers read the children's update matrices (the other depth parity of the arena, only
+// read during a launch), AtA and the plan's maps through pointers held in shared memory or computed per element; as generic loads each
+// one was consumed before the next was issued.
+template <typename T>
+__device__ __forceinline__ T front_ldg(const T* p) {
+#ifdef THB_SIMT_EMU
+  return *p;
+#else
+  return __ldg(p);
+#endif
+}
+
+// The gathers below issue the loads of several children before the first add: a child that does not reach an element contributes
+// -0.0, which is the exact identity of the addition (v + -0.0 == v for every v, -0.0 included), so each sum is bitwise the one of
+// adding only the children that reach the element, in list order.
+
 // ------------------------------------------------------------------------------------------------ fronts in shared memory
 // One CTA per (front, item).  Shared memory holds ONLY the panel: PN [w8 + b16 + 8][ldp] = pivot rows, identity padding up to w8 = w
 // rounded to 8, the border rows from row w8 on (b16 = b rounded to 16, zero padding), and Wd [8][20] = the inverse of the current
@@ -236,6 +252,57 @@ struct FrontChild {       // one child of the front this CTA works on (shared me
   const double* src;      // its update matrix for this item
   int ldg, lo, hi, uoff;  // leading dimension; range [lo, hi] of this front's rows the child reaches; its border vector's offset (f_u_off)
 };
+
+// Panel assembly: children q and q + 1 (those below nch) at the FRONT_PL panel elements (ii[u], jj[u]) (ii[u] < 0: none) -> x[c][u],
+// all loads issued before any is used
+__device__ __forceinline__ void front_panel_gather2(const FrontChild* ch, const int32_t* INV, int r, int nch, int q, const int* ii,
+                                                    const int* jj, double (&x)[2][FRONT_PL]) {
+#pragma unroll
+  for (int c = 0; c < 2; c++) {
+    int lo = r, hi = -1, ldg = 0;   // lo = r: nothing passes the range test below
+    const double* src = nullptr;
+    if (q + c < nch) { lo = ch[q + c].lo; hi = ch[q + c].hi; ldg = ch[q + c].ldg; src = ch[q + c].src; }
+    const int32_t* inv = INV + (q + c) * r;
+#pragma unroll
+    for (int u = 0; u < FRONT_PL; u++) {
+      x[c][u] = -0.0;
+      if (ii[u] >= lo && jj[u] <= hi) {
+        const int ci = inv[ii[u]], cj = inv[jj[u]];
+        if (ci >= 0 && cj >= 0) x[c][u] = front_ldg(src + (int64_t)ci * ldg + cj);
+      }
+    }
+  }
+}
+
+// Index of the lowest set bit of mask (mask != 0), which is cleared
+__device__ __forceinline__ int front_next_child(unsigned& mask) {
+#ifdef THB_SIMT_EMU
+  const int q = __builtin_ctz(mask);
+#else
+  const int q = __ffs(mask) - 1;
+#endif
+  mask &= mask - 1;
+  return q;
+}
+
+// Update-matrix tile: this lane's entries (rows li0, li0 + 8 and columns lj0 + {0, 1, 8, 9}, front-local) of child c, whose inverse map
+// is inv -> x, issued together
+__device__ __forceinline__ void front_tile_gather(const FrontChild& c, const int32_t* inv, int r, int li0, int lj0, double (&x)[2][2][2]) {
+  int ci[2], cj[2][2];
+#pragma unroll
+  for (int mi = 0; mi < 2; mi++) ci[mi] = (li0 + 8 * mi < r) ? inv[li0 + 8 * mi] : -1;
+#pragma unroll
+  for (int ni = 0; ni < 2; ni++)
+#pragma unroll
+    for (int u = 0; u < 2; u++) cj[ni][u] = (lj0 + 8 * ni + u < r) ? inv[lj0 + 8 * ni + u] : -1;
+#pragma unroll
+  for (int mi = 0; mi < 2; mi++)
+#pragma unroll
+    for (int ni = 0; ni < 2; ni++)
+#pragma unroll
+      for (int u = 0; u < 2; u++)
+        x[mi][ni][u] = (ci[mi] >= 0 && cj[ni][u] >= 0 && cj[ni][u] <= ci[mi]) ? front_ldg(c.src + (int64_t)ci[mi] * c.ldg + cj[ni][u]) : -0.0;
+}
 
 // ------------------------------------------------------------------------------------------------ forward elimination of one front
 // One warp: solve T y = u (lower triangular cw x cw, row stride ld) -- lane i owns u_i
@@ -379,21 +446,29 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
   double* Wd = PN + prow * ldp;             // [8][FRONT_WD_LD]
   FrontChild* ch = reinterpret_cast<FrontChild*>(Wd + 8 * FRONT_WD_LD);               // [FRONT_MAX_CHILDREN] (24 bytes each)
   int32_t* INV = reinterpret_cast<int32_t*>(Wd + 8 * FRONT_WD_LD + 3 * FRONT_MAX_CHILDREN);   // [nch][r] front row -> child row / -1
-  // ---- children descriptors and inverse maps go to shared memory (one round trip, then every lookup is on chip) ----
-  for (int q = 0; q < nch; q++) {
-    const int64_t* PC = p.pc + (int64_t)(c_begin + q) * 6;   // (cb_off, cb_ld, lo, hi, inv_off, u_off) of this child
-    const double* csrc = a.arena_child + item * p.arena_size + PC[0];
-    const int cld = (int)(PC[1] & 0xffffffffLL), cbc = (int)(PC[1] >> 32);
-    if (tid == 0) {
-      ch[q].src = csrc;
-      ch[q].ldg = cld;
-      ch[q].lo = (int)PC[2];
-      ch[q].hi = (int)PC[3];
-      ch[q].uoff = (int)PC[5];
+  // ---- children descriptors and inverse maps go to shared memory (one round trip, then every lookup is on chip): thread q reads child
+  // q's record, every thread the inverse-map offsets of all children, then its entries of all the maps -- no load waits for another
+  // child's ----
+  if (tid < nch) {
+    const int64_t* PC = p.pc + (int64_t)(c_begin + tid) * 6;   // (cb_off, cb_ld, lo, hi, inv_off, u_off) of this child
+    ch[tid].src = a.arena_child + item * p.arena_size + PC[0];
+    ch[tid].ldg = (int)(PC[1] & 0xffffffffLL);
+    ch[tid].lo = (int)PC[2];
+    ch[tid].hi = (int)PC[3];
+    ch[tid].uoff = (int)PC[5];
+  }
+  {
+    int64_t ioff[FRONT_MAX_CHILDREN];
+#pragma unroll
+    for (int q = 0; q < FRONT_MAX_CHILDREN; q++) ioff[q] = q < nch ? p.pc[(int64_t)(c_begin + q) * 6 + 4] : 0;
+    for (int l = tid; l < r; l += THREADS) {
+      int32_t iv[FRONT_MAX_CHILDREN];
+#pragma unroll
+      for (int q = 0; q < FRONT_MAX_CHILDREN; q++) iv[q] = q < nch ? front_ldg(p.c_inv + ioff[q] + l) : 0;
+#pragma unroll
+      for (int q = 0; q < FRONT_MAX_CHILDREN; q++)
+        if (q < nch) INV[q * r + l] = iv[q];
     }
-    const int32_t* inv = p.c_inv + PC[4];
-    for (int l = tid; l < r; l += THREADS) INV[q * r + l] = inv[l];
-    (void)cbc;
   }
   for (int e = tid; e < prow * ldp; e += THREADS) sm[e] = 0.0;
   int* next_tile = reinterpret_cast<int*>(Wd + 8);   // update-matrix tile counter, in a column of Wd's row padding that nothing else uses
@@ -429,7 +504,9 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
     const double al = a.alpha != nullptr ? a.alpha[item] : 0.0;
     const double be = a.beta != nullptr ? a.beta[item] : 0.0;
     const int total = r * w;
-    // FRONT_PL panel elements per thread and pass: their global loads (AtA entry + one per contributing child) are independent and in flight together
+    // FRONT_PL panel elements per thread and pass.  Loads are issued in groups and summed only after the whole group: the FRONT_PL
+    // pmap entries; the first two children's entries (they do not depend on pmap); the AtA values; then the next two children's
+    // entries, and so on.  The sums keep their order: AtA + damping, then the children in list order.
     for (int e0 = tid; e0 < total; e0 += FRONT_PL * THREADS) {
       int ii[FRONT_PL], jj[FRONT_PL];
       double v[FRONT_PL];
@@ -439,22 +516,26 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
         ii[u] = e / w;
         jj[u] = e - ii[u] * w;
         if (e >= total || jj[u] > ii[u]) ii[u] = -1;   // outside, or above the diagonal of the pivot block
-        v[u] = ii[u] >= 0 ? front_panel_in(a, Lg, f_panel_off, item, e) : 0.0;
+      }
+      int32_t m[FRONT_PL];
+#pragma unroll
+      for (int u = 0; u < FRONT_PL; u++) m[u] = (a.ata != nullptr && ii[u] >= 0) ? front_ldg(p.pmap + f_panel_off + e0 + u * THREADS) : -1;
+      double x[2][FRONT_PL];
+      front_panel_gather2(ch, INV, r, nch, 0, ii, jj, x);
+#pragma unroll
+      for (int u = 0; u < FRONT_PL; u++) {
+        if (a.ata != nullptr) v[u] = m[u] >= 0 ? front_ldg(a.ata + item * a.ata_stride + m[u]) : 0.0;
+        else v[u] = ii[u] >= 0 ? Lg[e0 + u * THREADS] : 0.0;
       }
 #pragma unroll
       for (int u = 0; u < FRONT_PL; u++)
         if (ii[u] >= 0 && ii[u] == jj[u]) v[u] = v[u] + (al * v[u] + be);   // linear/utils.py:14-33: diag <- diag (1 + alpha) + beta
-      for (int q = 0; q < nch; q++) {
-        const double* src = ch[q].src;
-        const int ldg = ch[q].ldg, lo = ch[q].lo, hi = ch[q].hi;
-        const int32_t* inv = INV + q * r;
+      for (int q = 0;;) {
 #pragma unroll
-        for (int u = 0; u < FRONT_PL; u++) {
-          if (ii[u] >= lo && jj[u] <= hi) {
-            const int ci = inv[ii[u]], cj = inv[jj[u]];
-            if (ci >= 0 && cj >= 0) v[u] += src[(int64_t)ci * ldg + cj];
-          }
-        }
+        for (int u = 0; u < FRONT_PL; u++) v[u] = (v[u] + x[0][u]) + x[1][u];
+        q += 2;
+        if (q >= nch) break;
+        front_panel_gather2(ch, INV, r, nch, q, ii, jj, x);
       }
 #pragma unroll
       for (int u = 0; u < FRONT_PL; u++)
@@ -526,48 +607,60 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) front_small_kernel(Fr
     while (R * (R + 1) / 2 > q) R--;
     if (R >= nmt) break;
     const int ct = q - R * (R + 1) / 2;
-    // gathered children first: their loads are in flight while the tensor pipe works on -P_I P_J^T
-    double gch[2][2][2] = {{{0.0, 0.0}, {0.0, 0.0}}, {{0.0, 0.0}, {0.0, 0.0}}};
+    // Per element: ((0 + first child) + next child ...) - P_I P_J^T, over the children that reach the tile, in list order.  With one
+    // such child its loads are issued before the DMMA loop and summed after it, in flight while the tensor pipe works on -P_I P_J^T.
+    // With more, they are summed before the loop (the first two children's loads issued together, then one child per round trip):
+    // the accumulators of the loop are not live yet, and under the 64-register cap there is no room for both.
+    unsigned reach = 0;   // warp-uniform: the children whose rows meet this tile
+    for (int qc = 0; qc < nch; qc++)
+      if (w + 16 * R + 15 >= ch[qc].lo && w + 16 * ct <= ch[qc].hi) reach |= 1u << qc;
+    double gch[2][2][2] = {{{-0.0, -0.0}, {-0.0, -0.0}}, {{-0.0, -0.0}, {-0.0, -0.0}}};
     const int li0 = w + 16 * R + lr, lj0 = w + 16 * ct + 2 * lc;   // front-local indices of this lane's 2 rows and 4 columns
-    for (int qc = 0; qc < nch; qc++) {
-      if (w + 16 * R + 15 >= ch[qc].lo && w + 16 * ct <= ch[qc].hi) {   // warp-uniform: does the child reach this tile at all
-        const int32_t* inv = INV + qc * r;
-        const double* src = ch[qc].src;
-        const int ldg = ch[qc].ldg;
-        int ci[2], cj[2][2];
+    if (reach != 0) {
+      const int qc = front_next_child(reach);
+      front_tile_gather(ch[qc], INV + qc * r, r, li0, lj0, gch);
+    }
+    const bool summed = reach != 0;   // more than one child: the sum is complete before the DMMA loop
+    for (bool first = true; reach != 0; first = false) {
+      const int qc = front_next_child(reach);
+      double x[2][2][2];
+      front_tile_gather(ch[qc], INV + qc * r, r, li0, lj0, x);
 #pragma unroll
-        for (int mi = 0; mi < 2; mi++) ci[mi] = (li0 + 8 * mi < r) ? inv[li0 + 8 * mi] : -1;
+      for (int mi = 0; mi < 2; mi++)
 #pragma unroll
         for (int ni = 0; ni < 2; ni++)
 #pragma unroll
-          for (int u = 0; u < 2; u++) cj[ni][u] = (lj0 + 8 * ni + u < r) ? inv[lj0 + 8 * ni + u] : -1;
-#pragma unroll
-        for (int mi = 0; mi < 2; mi++)
-#pragma unroll
-          for (int ni = 0; ni < 2; ni++)
-#pragma unroll
-            for (int u = 0; u < 2; u++)
-              if (ci[mi] >= 0 && cj[ni][u] >= 0 && cj[ni][u] <= ci[mi]) gch[mi][ni][u] += src[(int64_t)ci[mi] * ldg + cj[ni][u]];
-      }
+          for (int u = 0; u < 2; u++) gch[mi][ni][u] = (first ? 0.0 + gch[mi][ni][u] : gch[mi][ni][u]) + x[mi][ni][u];
     }
     double acc[2][2][2] = {{{0.0, 0.0}, {0.0, 0.0}}, {{0.0, 0.0}, {0.0, 0.0}}};
     const double* Pa = P + (16 * R + lr) * ldp + lc;
     const double* Pb = P + (16 * ct + lr) * ldp + lc;
-    for (int k4 = 0; k4 < w8; k4 += 4) {
-      const double a0 = Pa[k4], a1 = Pa[8 * ldp + k4];
-      const double b0 = Pb[k4], b1 = Pb[8 * ldp + k4];
-      front_mma884(acc[0][0][0], acc[0][0][1], a0, b0);
-      front_mma884(acc[0][1][0], acc[0][1][1], a0, b1);
-      front_mma884(acc[1][0][0], acc[1][0][1], a1, b0);
-      front_mma884(acc[1][1][0], acc[1][1][1], a1, b1);
+#pragma unroll 1   // w8 is a multiple of 8: no remainder loop, whose trip count spills
+    for (int k8 = 0; k8 < w8; k8 += 8) {
+#pragma unroll
+      for (int k4 = k8; k4 < k8 + 8; k4 += 4) {
+        const double a0 = Pa[k4], a1 = Pa[8 * ldp + k4];
+        const double b0 = Pb[k4], b1 = Pb[8 * ldp + k4];
+        front_mma884(acc[0][0][0], acc[0][0][1], a0, b0);
+        front_mma884(acc[0][1][0], acc[0][1][1], a0, b1);
+        front_mma884(acc[1][0][0], acc[1][0][1], a1, b0);
+        front_mma884(acc[1][1][0], acc[1][1][1], a1, b1);
+      }
+    }
+    if (!summed) {
+#pragma unroll
+      for (int mi = 0; mi < 2; mi++)
+#pragma unroll
+        for (int ni = 0; ni < 2; ni++)
+#pragma unroll
+          for (int u = 0; u < 2; u++) gch[mi][ni][u] = 0.0 + gch[mi][ni][u];
     }
 #pragma unroll
     for (int mi = 0; mi < 2; mi++)
 #pragma unroll
-      for (int ni = 0; ni < 2; ni++) {
-        acc[mi][ni][0] = gch[mi][ni][0] - acc[mi][ni][0];
-        acc[mi][ni][1] = gch[mi][ni][1] - acc[mi][ni][1];
-      }
+      for (int ni = 0; ni < 2; ni++)
+#pragma unroll
+        for (int u = 0; u < 2; u++) acc[mi][ni][u] = gch[mi][ni][u] - acc[mi][ni][u];
 #pragma unroll
     for (int mi = 0; mi < 2; mi++) {
       const int i = 16 * R + 8 * mi + lr;
@@ -591,8 +684,9 @@ constexpr int ASM_ROWS = 16, ASM_THREADS = 256;
 __device__ __forceinline__ int front_map_big(int l, int w, int wpad) { return l < w ? l : wpad + (l - w); }
 
 // grid: x = item, y = row tile (np / ASM_ROWS).  Builds rows [R0, R0 + ASM_ROWS) of the padded front matrix F (np x np, row-major):
-// zeros, identity on the padding, the panel's AtA entries (+ damping), the children's update matrices; written once.
-__global__ void __launch_bounds__(ASM_THREADS) front_assemble_kernel(FrontArgs a, int t) {
+// zeros, identity on the padding, the panel's AtA entries (+ damping), the children's update matrices; written once.  Four CTAs per SM
+// (64 registers): the grouped loads of the gather form would take 72 and leave room for three.
+__global__ void __launch_bounds__(ASM_THREADS, 4) front_assemble_kernel(FrontArgs a, int t) {
   extern __shared__ double sm[];
   const thb_front_plan& p = a.p;
   const int tid = threadIdx.x;
@@ -610,7 +704,7 @@ __global__ void __launch_bounds__(ASM_THREADS) front_assemble_kernel(FrontArgs a
     const double beg = a.beta != nullptr ? a.beta[item] : 0.0;
     double* Fg = a.arena_cur + item * p.arena_size + p.f_fr_off[t] + (int64_t)R0 * np;
     // children descriptors once per CTA (the per-element chain child_list -> c_inv_ptr -> inv -> update matrix was four dependent
-    // global loads per child and element); then four entries per thread and pass, their loads in flight together
+    // global loads per child and element); then four entries per thread and pass
     __shared__ const double* s_src[FRONT_MAX_CHILDREN];
     __shared__ const int32_t* s_inv[FRONT_MAX_CHILDREN];
     __shared__ int s_ld[FRONT_MAX_CHILDREN];
@@ -623,8 +717,30 @@ __global__ void __launch_bounds__(ASM_THREADS) front_assemble_kernel(FrontArgs a
     __syncthreads();
     const int64_t poff = p.f_panel_off[t];
     const int total = ASM_ROWS * nc;
+    // children two at a time: the inverse-map entries of both, then their update-matrix entries (-0.0 where a child does not reach the
+    // element), each group issued before any of it is used
+    auto gather2 = [&](int q, const int (&li)[4], const int (&lj)[4], double (&x)[2][4]) {
+      int ci[2][4], cj[2][4];
+#pragma unroll
+      for (int c = 0; c < 2; c++) {
+        const int32_t* inv = q + c < n_children ? s_inv[q + c] : nullptr;
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+          ci[c][u] = (inv != nullptr && li[u] >= 0) ? front_ldg(inv + li[u]) : -1;
+          cj[c][u] = (inv != nullptr && li[u] >= 0) ? front_ldg(inv + lj[u]) : -1;
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < 2; c++) {
+        const double* src = q + c < n_children ? s_src[q + c] : nullptr;
+        const int ldg = q + c < n_children ? s_ld[q + c] : 0;
+#pragma unroll
+        for (int u = 0; u < 4; u++) x[c][u] = (ci[c][u] >= 0 && cj[c][u] >= 0) ? front_ldg(src + (int64_t)ci[c][u] * ldg + cj[c][u]) : -0.0;
+      }
+    };
     for (int e0 = tid; e0 < total; e0 += 4 * ASM_THREADS) {
       int li[4], lj[4];
+      int pe[4];   // panel element of the entry (its AtA value), or -1
       double v[4];
 #pragma unroll
       for (int u = 0; u < 4; u++) {
@@ -634,6 +750,7 @@ __global__ void __launch_bounds__(ASM_THREADS) front_assemble_kernel(FrontArgs a
         li[u] = fr < w ? fr : ((fr >= wpad && fr - wpad + w < r) ? fr - wpad + w : -1);
         lj[u] = fc < w ? fc : ((fc >= wpad && fc - wpad + w < r) ? fc - wpad + w : -1);
         v[u] = 0.0;
+        pe[u] = -1;
         if (e >= total) {
           li[u] = lj[u] = -2;                         // past the end: nothing to store
         } else if (li[u] < 0 || lj[u] < 0) {
@@ -642,25 +759,28 @@ __global__ void __launch_bounds__(ASM_THREADS) front_assemble_kernel(FrontArgs a
         } else if (lj[u] > li[u]) {
           li[u] = -1;                                 // above the diagonal: zero
         } else if (lj[u] < w) {
-          v[u] = front_panel_in(a, Lgg, poff, item, (int64_t)li[u] * w + lj[u]);
+          pe[u] = li[u] * w + lj[u];
         }
+      }
+      int32_t m[4];
+#pragma unroll
+      for (int u = 0; u < 4; u++) m[u] = (a.ata != nullptr && pe[u] >= 0) ? front_ldg(p.pmap + poff + pe[u]) : -1;
+      double x[2][4];
+      gather2(0, li, lj, x);
+#pragma unroll
+      for (int u = 0; u < 4; u++) {
+        if (a.ata != nullptr) { if (m[u] >= 0) v[u] = front_ldg(a.ata + item * a.ata_stride + m[u]); }
+        else if (pe[u] >= 0) v[u] = Lgg[pe[u]];
       }
 #pragma unroll
       for (int u = 0; u < 4; u++)
         if (li[u] >= 0 && li[u] == lj[u] && lj[u] < w) v[u] = v[u] + (alg * v[u] + beg);
-      for (int q = 0; q < n_children; q++) {
-        const double* src = s_src[q];
-        const int32_t* inv = s_inv[q];
-        const int ldg = s_ld[q];
-        int ci[4], cj[4];
+      for (int q = 0;;) {
 #pragma unroll
-        for (int u = 0; u < 4; u++) {
-          ci[u] = li[u] >= 0 ? inv[li[u]] : -1;
-          cj[u] = li[u] >= 0 ? inv[lj[u]] : -1;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; u++)
-          if (ci[u] >= 0 && cj[u] >= 0) v[u] += src[(int64_t)ci[u] * ldg + cj[u]];
+        for (int u = 0; u < 4; u++) v[u] = (v[u] + x[0][u]) + x[1][u];
+        q += 2;
+        if (q >= n_children) break;
+        gather2(q, li, lj, x);
       }
 #pragma unroll
       for (int u = 0; u < 4; u++) {
