@@ -15,10 +15,12 @@ Problem description ("spec"), batch-first like the reference:
                   "aux": ndarray [B or 1, ...]   (measurement / target),
                   "weight": ("diag", ndarray [B or 1, dim]) | ("scale", ndarray [B or 1, 1])}, ...]  # objective order
     }
+The motion-planning and planar-pushing kinds (collision, double_integrator, hinge, nonholonomic, qsp, eoc) and the GP weight
+("gp", Qc_inv [B or 1, D, D], dt [B or 1, 1]) are described in oracle/embodied.py.
 """
 import numpy as np
 
-from . import lie
+from . import embodied, lie
 
 _GROUP = {
     "SE3": dict(dof=6, inverse=lie.se3_inverse, compose=lie.se3_compose, jlog=lie.se3_jlog,
@@ -66,9 +68,14 @@ def local_error_jacobians(group, X, T, want_jac=True):
 
 
 def weight_jacobians_error(weight, jacs, err):
-    """theseus/core/cost_weight.py:81-90 (Scale), :125-136 (Diagonal)."""
-    kind, w = weight
+    """theseus/core/cost_weight.py:81-90 (Scale), :125-136 (Diagonal); GPCostWeight (embodied/motionmodel/double_integrator.py:154-170):
+    W e and W J with W the factor of embodied.gp_weight."""
+    kind, w = weight[0], weight[1]
     B = err.shape[0]
+    if kind == "gp":
+        W = embodied.gp_weight(_bcast(np.asarray(w, dtype=err.dtype), B), _bcast(np.asarray(weight[2], dtype=err.dtype), B))
+        e = (W @ err[:, :, None])[:, :, 0]
+        return (None if jacs is None else [W @ J for J in jacs]), e
     w = _bcast(np.asarray(w, dtype=err.dtype), B)
     if kind == "scale":
         w = w.reshape(B, 1)
@@ -155,6 +162,8 @@ def robust_apply(robust, jacs, e, flatten_dims=False):
 
 
 def cost_dim(spec, cost):
+    if cost["kind"] in embodied.KINDS:
+        return embodied.cost_dim(spec, cost)
     if cost["kind"] == "reproj":
         return 2
     if cost.get("group") == "Vector":
@@ -169,10 +178,16 @@ def eval_costs(spec, values, want_jac=True):
     B = values[0].shape[0]
     dt = spec["dtype"]
     groups = {}
+    out = [None] * len(spec["costs"])
     for f, c in enumerate(spec["costs"]):
+        if c["kind"] in embodied.KINDS:      # one cost function at a time (float64 throughout: no stacking order to follow)
+            if c.get("robust") is not None:
+                raise NotImplementedError(f"robust loss on a {c['kind']} cost function")
+            jac_list, err = embodied.cost_jacobians_error(spec, c, values, want_jac)
+            out[f] = weight_jacobians_error(c["weight"], jac_list, err.astype(dt))
+            continue
         groups.setdefault((c["kind"], c.get("group", "-") + (str(spec["vars"][c["vars"][0]]["dof"]) if c.get("group") == "Vector" else ""),
                            c["weight"][0]), []).append(f)
-    out = [None] * len(spec["costs"])
 
     def put(f, jac_list, err):
         c = spec["costs"][f]

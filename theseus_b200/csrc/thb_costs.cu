@@ -785,42 +785,47 @@ __device__ __forceinline__ void mp_cost(const GroupDev<T>& g, int k, int64_t b, 
   }
 }
 
-// The cost weight of one (k, b): per-row factors (Scale / Diagonal) or the GP weight's upper factor L^T = (chol S)^T (x) (chol Qc_inv)^T,
-// S = [[12/dt^3, -6/dt^2], [-6/dt^2, 4/dt]] (double_integrator.py:131-152): L^T = [[a U, b U], [0, c U]] with U = chol(Qc_inv)^T.
+// The cost weight of one (k, b): per-row factors (Scale / Diagonal) or the GP weight's upper factor U = cholesky(W^T)^T of
+// W = [[12/dt^3 Q, -6/dt^2 Q], [-6/dt^2 Q, 4/dt Q]], Q = Qc_inv (double_integrator.py:131-152).  The Cholesky reads only the lower
+// triangle of W^T, i.e. M(i, j) = W(j, i) for i >= j: for a non-symmetric Q that matrix is not S (x) Q of either triangle, so the
+// 2D x 2D factor is formed here in full (at most 6 x 6) rather than as chol(S)^T (x) chol(Q)^T.
 template <typename T, int DIM, int D> struct MpWeight {
   bool gp;
   T w[DIM];
-  T a, bq, c, U[D * D];
+  T U[DIM * DIM];   // GP: U(p, q) for q >= p
 
   __device__ __forceinline__ bool load(const GroupDev<T>& g, int k, int64_t b) {
     gp = g.weight_kind == THB_WEIGHT_GP;
-    if (!gp) return load_weight<T, DIM>(g, k, b, w);
-    const T* Q = g.w[k] + (int64_t)g.bstride[k * 4 + 3] * b;
-    const T dt = mp_aux(g, 1, k, b)[0];
-    T L[D * D];
+    if constexpr (DIM == 2 * D) {
+      if (gp) {
+        const T* Q = g.w[k] + (int64_t)g.bstride[k * 4 + 3] * b;
+        const T dt = mp_aux(g, 1, k, b)[0];
+        const T s00 = T(12) / (dt * dt * dt), s01 = T(-6) / (dt * dt), s11 = T(4) / dt;   // S = [[s00, s01], [s01, s11]]
+        auto M = [&](int i, int j) {   // i >= j: W(j, i)
+          const int blk = j / D + i / D;
+          return (blk == 0 ? s00 : (blk == 1 ? s01 : s11)) * Q[(j % D) * D + (i % D)];
+        };
+        // U^T U = M column by column: U(j, j) = sqrt(M(j, j) - sum_q U(q, j)^2), U(j, i) = (M(i, j) - sum_q U(q, i) U(q, j)) / U(j, j)
 #pragma unroll
-    for (int j = 0; j < D; j++) {
-      T s = Q[j * D + j];
+        for (int j = 0; j < DIM; j++) {
+          T d = M(j, j);
 #pragma unroll
-      for (int q = 0; q < j; q++) s -= L[j * D + q] * L[j * D + q];
-      const T ljj = t_sqrt(s);
-      L[j * D + j] = ljj;
+          for (int q = 0; q < j; q++) d -= U[q * DIM + j] * U[q * DIM + j];
+          const T ujj = t_sqrt(d);
+          const T rjj = T(1) / ujj;   // one division per column, the row scaled by it (as LAPACK's potf2 does)
+          U[j * DIM + j] = ujj;
 #pragma unroll
-      for (int i = j + 1; i < D; i++) {
-        T t = Q[i * D + j];
+          for (int i = j + 1; i < DIM; i++) {
+            T t = M(i, j);
 #pragma unroll
-        for (int q = 0; q < j; q++) t -= L[i * D + q] * L[j * D + q];
-        L[i * D + j] = t / ljj;
+            for (int q = 0; q < j; q++) t -= U[q * DIM + i] * U[q * DIM + j];
+            U[j * DIM + i] = t * rjj;
+          }
+        }
+        return false;
       }
     }
-#pragma unroll
-    for (int p = 0; p < D; p++)
-#pragma unroll
-      for (int q = 0; q < D; q++) U[p * D + q] = (q >= p) ? L[q * D + p] : T(0);
-    a = t_sqrt(T(12) / (dt * dt * dt));
-    bq = (T(-6) / (dt * dt)) / a;
-    c = t_sqrt(T(4) / dt - bq * bq);
-    return false;
+    return load_weight<T, DIM>(g, k, b, w);   // (mp_dof admits a GP weight only for the DoubleIntegrator kinds, DIM = 2 D)
   }
   // columns 0..ncols-1 of the DIM x ld row block v (ncols = 1, ld = 1: a vector) <- W v
   __device__ __forceinline__ void apply(T* v, int ld, int ncols) const {
@@ -832,19 +837,13 @@ template <typename T, int DIM, int D> struct MpWeight {
     }
     if constexpr (DIM == 2 * D) {
       for (int j = 0; j < ncols; j++) {
-        T top[D], bot[D];
+        // row p reads rows q >= p only: overwriting in increasing p is safe
 #pragma unroll
-        for (int p = 0; p < D; p++) { top[p] = v[p * ld + j]; bot[p] = v[(D + p) * ld + j]; }
+        for (int p = 0; p < DIM; p++) {
+          T acc = T(0);
 #pragma unroll
-        for (int p = 0; p < D; p++) {
-          T st = T(0), sb = T(0);
-#pragma unroll
-          for (int q = p; q < D; q++) {
-            st += U[p * D + q] * (a * top[q] + bq * bot[q]);
-            sb += U[p * D + q] * bot[q];
-          }
-          v[p * ld + j] = st;
-          v[(D + p) * ld + j] = c * sb;
+          for (int q = p; q < DIM; q++) acc += U[p * DIM + q] * v[q * ld + j];
+          v[p * ld + j] = acc;
         }
       }
     }
