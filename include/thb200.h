@@ -205,11 +205,29 @@ typedef struct thb_gram_plan {
   int64_t num_blocks;         /* NB */
   const int32_t* blk_rows;    /* device [NB] rows of the block (its columns are blk_ld for packed block storage) */
   const int32_t* blk_cols;    /* device [NB] columns of the block */
-  /* block-per-thread Gram kernels (one thread = one whole block of one item): blocks grouped by shape.  num_segments == 0 (some block
-   * shape outside {1,2,3,6} x {1,2,3,6}): the entry-per-thread kernel runs instead. */
+  /* block-per-thread Gram kernels (one thread = one whole block of one item), for plans without groups: blocks grouped by shape.
+   * num_segments == 0 (some block shape outside {1,2,3,6} x {1,2,3,6}): the entry-per-thread kernel runs instead. */
   int64_t num_segments;
   const int32_t* segments;    /* HOST [num_segments,4] = (rows, cols, begin, end) into blk_order */
   const int32_t* blk_order;   /* device [NB] block ids sorted by shape */
+  /* staged Gram kernel: one CTA per (batch item, group of consecutive variables).  It copies the rows of A and b of every cost
+   * function the group touches to shared memory, then forms the group's blocks (those whose row variable it holds), Atb and diag
+   * from there.  num_groups == 0 (a variable's cost functions do not fit the budget): the kernels above run instead. */
+  int64_t num_groups;         /* G */
+  int64_t stage_elems;        /* scalars of shared memory the largest group stages */
+  const int32_t* stage_ptr;   /* device [G+1] CSR pointer into the st_* arrays */
+  const int64_t* st_off;      /* device [NS] A_val offset of the staged cost function's first row */
+  const int32_t* st_len;      /* device [NS] its rows x stride */
+  const int32_t* st_row0;     /* device [NS] its first row in b */
+  const int32_t* st_dim;      /* device [NS] its rows */
+  const int32_t* st_soff;     /* device [NS] shared-memory offset of its A rows (its b rows follow them) */
+  const int32_t* task_ptr;    /* device [G+1] CSR pointer into the task arrays */
+  const int32_t* task_blk;    /* device [NT] block of the task: one row of one block, up to 6 columns */
+  const int32_t* task_pq;     /* device [NT] (row << 16) | first column */
+  const int32_t* grp_col;     /* device [G+1] the group's columns are [grp_col[g], grp_col[g+1]) */
+  const int32_t* c_soff;      /* device [NC] shared-memory offset of the contribution's first row */
+  const int32_t* cc_soff;     /* device [NCC] shared-memory offset of (first row, this column) */
+  const int32_t* cc_sb;       /* device [NCC] shared-memory offset of the cost function's first b row */
 } thb_gram_plan;
 
 /* out[b*out_bstride + ...] receives the blocks (dense AtA: out_bstride = n*n, caller pre-zeroes via

@@ -27,13 +27,18 @@ class VarTable(C.Structure):
     _fields_ = [("N", c_i32), ("x", c_vp), ("out", c_vp), ("kind", c_vp), ("col", c_vp), ("dof", c_vp)]
 
 
+_GRAM_STAGED = ("stage_ptr", "st_off", "st_len", "st_row0", "st_dim", "st_soff", "task_ptr", "task_blk", "task_pq", "grp_col", "c_soff",
+                "cc_soff", "cc_sb")
+
+
 class GramPlan(C.Structure):
     _fields_ = [("num_entries", c_i64), ("ent_blk", c_vp), ("ent_p", c_vp), ("ent_q", c_vp),
                 ("blk_out", c_vp), ("blk_ld", c_vp), ("blk_mirror", c_vp), ("blk_cptr", c_vp),
                 ("c_off", c_vp), ("c_stride", c_vp), ("c_rows", c_vp), ("c_bpa", c_vp), ("c_bpb", c_vp),
                 ("n", c_i64), ("col_cptr", c_vp), ("cc_off", c_vp), ("cc_stride", c_vp), ("cc_rows", c_vp),
                 ("cc_row0", c_vp), ("num_blocks", c_i64), ("blk_rows", c_vp), ("blk_cols", c_vp),
-                ("num_segments", c_i64), ("segments", c_vp), ("blk_order", c_vp)]
+                ("num_segments", c_i64), ("segments", c_vp), ("blk_order", c_vp),
+                ("num_groups", c_i64), ("stage_elems", c_i64)] + [(k, c_vp) for k in _GRAM_STAGED]
 
 
 def make_gram_plan(arrs, dev):
@@ -47,7 +52,8 @@ def make_gram_plan(arrs, dev):
         cc_off=dev["cc_off"].data_ptr(), cc_stride=dev["cc_stride"].data_ptr(), cc_rows=dev["cc_rows"].data_ptr(),
         cc_row0=dev["cc_row0"].data_ptr(), num_blocks=int(arrs["blk_out"].shape[0]), blk_rows=dev["blk_rows"].data_ptr(),
         blk_cols=dev["blk_cols"].data_ptr(), num_segments=int(arrs["segments"].shape[0]), segments=arrs["segments"].ctypes.data,
-        blk_order=dev["blk_order"].data_ptr())
+        blk_order=dev["blk_order"].data_ptr(), num_groups=int(arrs["num_groups"]), stage_elems=int(arrs["stage_elems"]),
+        **{k: dev[k].data_ptr() for k in _GRAM_STAGED})
 
 
 class SparsePlanStruct(C.Structure):

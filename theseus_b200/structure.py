@@ -117,11 +117,45 @@ def lower_blocks(s: Structure, pos=None):
     return blocks, contribs
 
 
-def build_gram_plan(s: Structure, out_offsets=None, pos=None):
+GRAM_STAGE_ELEMS = 5120     # shared-memory budget of one staged Gram CTA, in scalars (40 KB of fp64: five CTAs per SM)
+GRAM_STAGE_COLS = 6         # columns of a block one thread of the staged kernel accumulates (thb_gram.cu: STAGE_COLS)
+
+
+def _gram_groups(s: Structure, per_var, budget):
+    """Consecutive variables (structure order) cut into groups whose cost functions' rows of A and b fit `budget` scalars.
+    Returns (group of each variable, [staged cost functions of each group, ascending]), or None when one variable alone does not fit."""
+    if budget <= 0:
+        return None
+    size = s.cost_dims * (s.stride + 1)
+    group_of = np.zeros(len(s.var_dims), dtype=np.int64)
+    groups, cur, used = [], set(), 0
+    for v in range(len(s.var_dims)):
+        new = {f for f, _ in per_var[v]} - cur
+        add = int(sum(size[f] for f in new))
+        if cur and used + add > budget:
+            groups.append(sorted(cur))
+            cur, used = set(), 0
+            new = {f for f, _ in per_var[v]}
+            add = int(sum(size[f] for f in new))
+        if add > budget:
+            return None
+        cur |= new
+        used += add
+        group_of[v] = len(groups)
+    if len(s.var_dims):
+        groups.append(sorted(cur))
+    return group_of, groups
+
+
+def build_gram_plan(s: Structure, out_offsets=None, pos=None, stage_budget=GRAM_STAGE_ELEMS):
     """Arrays of the thb_gram_plan struct (include/thb200.h).
 
     out_offsets: None -> dense AtA [n,n] row-major (lower blocks + mirrored upper blocks);
                  or a callable (i, j) -> (offset, ld, mirror_offset) for block-sparse factor storage.
+    stage_budget: scalars of A and b one CTA of the staged kernel may hold in shared memory.  The variables are cut into groups
+                 whose cost functions fit it; a variable whose cost functions alone do not fit (or stage_budget=0) leaves the plan
+                 without groups, and thb_gram_f64 then runs the block-per-thread kernels (every block shape in
+                 {1,2,3,6} x {1,2,3,6}) or the entry-per-thread one.
     """
     blocks, contribs = lower_blocks(s, pos)
     n = s.num_cols
@@ -173,7 +207,54 @@ def build_gram_plan(s: Structure, out_offsets=None, pos=None):
     def cat(lst, dt):
         return np.concatenate(lst).astype(dt) if lst else np.zeros(0, dtype=dt)
 
-    # blocks grouped by shape for the block-per-thread kernels (thb_gram.cu: gram_block_kernel<DI, DJ>)
+    # staged kernel (thb_gram.cu: gram_staged_kernel): per group of variables, the cost functions whose rows it copies to shared
+    # memory (A rows, then b rows, ascending cost function), the work items (one row of one owned block, up to GRAM_STAGE_COLS
+    # columns) and its columns; every contribution's shared-memory offset.  A block belongs to the group of its row variable.
+    grouping = _gram_groups(s, per_var, stage_budget)
+    stage_ptr, st_off, st_len, st_row0, st_dim, st_soff = [0], [], [], [], [], []
+    task_ptr, task_blk, task_pq, grp_col = [0], [], [], [0]
+    c_soff, cc_soff, cc_sb = np.zeros(len(c_off), np.int32), np.zeros(len(cc_off), np.int32), np.zeros(len(cc_off), np.int32)
+    stage_elems = 0
+    if grouping is not None:
+        group_of, groups = grouping
+        soff = []
+        for fs in groups:
+            at, o = {}, 0
+            for f in fs:
+                at[f] = o
+                st_off.append(int(s.row_block_starts[f]))
+                st_len.append(int(s.cost_dims[f] * s.stride[f]))
+                st_row0.append(int(s.cost_row0[f]))
+                st_dim.append(int(s.cost_dims[f]))
+                st_soff.append(o)
+                o += int(s.cost_dims[f] * (s.stride[f] + 1))
+            soff.append(at)
+            stage_ptr.append(len(st_off))
+            stage_elems = max(stage_elems, o)
+        owned = [[] for _ in groups]
+        for k, (i, j) in enumerate(blocks):
+            g = int(group_of[i])
+            owned[g].append(k)
+            for c, (f, a, b) in zip(range(blk_cptr[k], blk_cptr[k + 1]), contribs[k]):
+                c_soff[c] = soff[g][f]
+        for g, ks in enumerate(owned):
+            for k in ks:
+                for p in range(blk_rows[k]):
+                    for q0 in range(0, blk_cols[k], GRAM_STAGE_COLS):
+                        task_blk.append(k)
+                        task_pq.append((p << 16) | q0)
+            task_ptr.append(len(task_blk))
+        cc = 0
+        for i in range(len(s.var_dims)):
+            g = int(group_of[i])
+            for pc in range(int(s.var_dims[i])):
+                for (f, a) in per_var[i]:
+                    cc_soff[cc] = soff[g][f] + int(s.block_pointers[f][a]) + pc
+                    cc_sb[cc] = soff[g][f] + int(s.cost_dims[f] * s.stride[f])
+                    cc += 1
+            if i + 1 == len(s.var_dims) or group_of[i + 1] != g:
+                grp_col.append(int(s.var_start_cols[i] + s.var_dims[i]))
+    # blocks grouped by shape for the block-per-thread kernels that serve plans without groups (thb_gram.cu: gram_block_kernel<DI, DJ>)
     shapes = sorted(set(zip(blk_rows, blk_cols)))
     if all(di in (1, 2, 3, 6) and dj in (1, 2, 3, 6) for di, dj in shapes):
         order, segments = [], []
@@ -187,6 +268,11 @@ def build_gram_plan(s: Structure, out_offsets=None, pos=None):
         blk_order, segments = np.zeros(1, dtype=np.int32), np.zeros((0, 4), dtype=np.int32)
     return dict(
         blk_order=blk_order, segments=segments,
+        num_groups=len(stage_ptr) - 1, stage_elems=stage_elems,
+        stage_ptr=np.array(stage_ptr, dtype=np.int32), st_off=np.array(st_off, dtype=np.int64), st_len=np.array(st_len, dtype=np.int32),
+        st_row0=np.array(st_row0, dtype=np.int32), st_dim=np.array(st_dim, dtype=np.int32), st_soff=np.array(st_soff, dtype=np.int32),
+        task_ptr=np.array(task_ptr, dtype=np.int32), task_blk=np.array(task_blk, dtype=np.int32), task_pq=np.array(task_pq, dtype=np.int32),
+        grp_col=np.array(grp_col, dtype=np.int32), c_soff=c_soff, cc_soff=cc_soff, cc_sb=cc_sb,
         ent_blk=cat(ent_blk, np.int32), ent_p=cat(ent_p, np.int16), ent_q=cat(ent_q, np.int16),
         blk_out=np.array(blk_out, dtype=np.int64), blk_ld=np.array(blk_ld, dtype=np.int32),
         blk_mirror=np.array(blk_mirror, dtype=np.int64), blk_cptr=np.array(blk_cptr, dtype=np.int32),
