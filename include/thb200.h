@@ -478,9 +478,9 @@ int thb_gram_dense_f64(const double* A, double* AtA, int64_t B, int64_t m, int64
  *     [B, data_size]); the caller zero-fills first.  Damping (alpha, beta) is applied while a panel is loaded.
  *   update matrices (Schur complements) live for one depth step in arena [2][B][arena_size] (parity = depth & 1):
  *     small fronts: lower triangle of a b x b matrix at f_cb_off[t], leading dimension f_cb_ld[t];
- *     big fronts (f_class == 3): the whole padded front matrix F [np x np] at f_fr_off[t] (pivot columns padded to f_wpad[t],
- *     a multiple of 64, identity on the padding), factored in place by the DMMA dense kernel in partial mode
- *     (thb_potrf_partial_inplace_f64); its trailing block IS the update matrix (f_cb_off / f_cb_ld point into it).
+ *     big fronts (f_class == 3): the region of the padded front matrix F [np x np] at f_fr_off[t] (pivot columns padded to f_wpad[t],
+ *     a multiple of 64); the DMMA dense kernel in partial mode factors the front straight into its panel and writes the trailing
+ *     block -- the update matrix -- there (f_cb_off / f_cb_ld point into it).
  *   child -> parent maps: f_rel[rel_ptr[c] .. rel_ptr[c+1]) = local row index in the parent front of child c's border rows.
  * `launches` is a HOST array [num_launches][12] (int64) in factorisation order (deepest fronts first):
  *   (depth, class, begin, count [into sched], dynamic smem bytes of the factor kernel, largest front of the launch [np for class 3],

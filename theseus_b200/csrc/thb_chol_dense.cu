@@ -21,7 +21,13 @@
 // Solve: x = M^-1 rhs with the stored W_j (triangular solves become mat-vecs), one CTA per matrix, HBM-bound.
 //
 // wgmma has no fp64 kind; the FP64 tensor pipe of sm_90a is reached with mma.sync DMMA (m8n8k4).
+#include <stdlib.h>
+
 #include "thb_common.cuh"
+
+#ifndef THB_CHOL_GROUP_DEFAULT
+#define THB_CHOL_GROUP_DEFAULT (1LL << 40)
+#endif
 
 namespace thb {
 
@@ -70,6 +76,15 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src)
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem_src));
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
+// with src_bytes < 16 (0 or 8) the rest of the 16 bytes is zero-filled
+__device__ __forceinline__ void cp_async16_zfill(void* smem_dst, const void* gmem_src, int src_bytes) {
+  const unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem_src), "r"(src_bytes));
+}
+__device__ __forceinline__ void cp_async8_zfill(void* smem_dst, const void* gmem_src, int src_bytes) {
+  const unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;\n" ::"r"(s), "l"(gmem_src), "r"(src_bytes));
+}
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 // stage one [ROWS x KB] operand tile: ROWS consecutive rows of a row-major matrix (leading dimension ld), columns k0..k0+KB
@@ -216,9 +231,9 @@ __device__ __forceinline__ int block_factor_invert(double* __restrict__ T, doubl
 }
 
 // All 256 threads.  T: the 64x64 diagonal block inside the C tile (row stride SC), Wd: scratch [2][32][SB32],
-// Lg/ldl: where L_jj goes in global memory, Wg: where W = L_jj^-1 goes (row-major 64x64).
+// Lg/ldl: where L_jj goes in global memory (its first lim rows and columns), Wg: where W = L_jj^-1 goes (row-major 64x64).
 __device__ __noinline__ int diag64_factor_invert(double* __restrict__ T, double* __restrict__ Wd, double* __restrict__ Lg, int64_t ldl,
-                                                 double* __restrict__ Wg) {
+                                                 int lim, double* __restrict__ Wg) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int lr = lane >> 2, lc = lane & 3;
   __shared__ int s_fail;
@@ -267,7 +282,7 @@ __device__ __noinline__ int diag64_factor_invert(double* __restrict__ T, double*
   // ---- store L_jj (lower part; zeros above) ----
   for (int e = tid; e < 64 * 64; e += CHOL_THREADS) {
     const int r = e >> 6, c = e & 63;
-    Lg[(int64_t)r * ldl + c] = (c <= r) ? T[r * SC + c] : 0.0;
+    if (r < lim && c < lim) Lg[(int64_t)r * ldl + c] = (c <= r) ? T[r * SC + c] : 0.0;
   }
   __syncthreads();
   // ---- inverse: diagonal blocks <- W_kk (explicit zeros above the diagonal), then W10 = -(W11 L10) W00 ----
@@ -306,7 +321,6 @@ struct CholArgs {
   double* W;           // [B,nb,64,64] (nb = np/64)
   int* flags;          // [B,nb]      W_j ready
   int* done;           // [B,ntr]     number of finished block columns of each 128-row tile
-  const int64_t* col_start;  // [nb+1] first CTA index of every block column (one launch covers the whole factorisation)
   int32_t* info;       // [B]
   int64_t B, n, np;
   int nb, ntr;
@@ -318,7 +332,40 @@ struct CholArgs {
   int k_lim;           // partial mode: KB-steps of the k loop that hold real pivot columns (the identity padding of the last pivot
                        // block column contributes nothing to the rows below it); the full factorisation uses nb * TN / KB
   int n_real;          // partial mode: rows / columns >= n_real are padding (tiles that lie entirely there are skipped)
+  int group;           // tickets go to groups of `group` matrices, one group after the other (B: one group)
+  ThbCholDirect d;     // partial mode on a big front of the multifrontal factor (d.fd != null): the initial tiles are gathered from
+                       // AtA and the children's update matrices, the pivot columns' L goes to the front's panel and is read from there
 };
+
+// Direct mode: front row (= row of its panel) of row fr of the padded front matrix, or -1 in the padding
+__device__ __forceinline__ int direct_row(const ThbCholDirect& d, int fr) {
+  return fr < d.w ? fr : ((fr >= d.wpad && fr - d.wpad < d.b) ? fr - d.wpad + d.w : -1);
+}
+
+// Direct mode: stage [ROWS x KB] of L from the panel (row-major, ld w): rows row0.. of the padded front matrix, columns k0..k0+KB.
+// Padding rows and columns >= w are zero-filled.  Of the values the in-place form reads there (identity / zeros of the padding, L of
+// the padding rows and of the columns between w and the next multiple of KB), the only ones that are not +0.0 multiply into rows or
+// columns of the padding, which are never stored; a +0.0 product added to a real entry leaves it bitwise unchanged.
+template <int ROWS>
+__device__ __forceinline__ void load_panel_tile(double* dst, const double* __restrict__ Pn, const ThbCholDirect& d, int row0, int k0, int tid) {
+  constexpr int CPR = KB / 2;
+#pragma unroll
+  for (int q = 0; q < (ROWS * CPR) / CHOL_THREADS; q++) {
+    const int chunk = tid + q * CHOL_THREADS;
+    const int row = chunk / CPR, cc = chunk % CPR;
+    const int pr = direct_row(d, row0 + row), k = k0 + cc * 2;
+    double* s = dst + row * SA + cc * 2;
+    const double* g = Pn + (int64_t)(pr >= 0 ? pr : 0) * d.w + k;
+    if ((d.w & 1) == 0) {   // every row 16-byte aligned (panels are)
+      const bool ok = pr >= 0 && k < d.w;
+      cp_async16_zfill(s, ok ? g : Pn, ok ? 16 : 0);
+    } else {
+      const bool ok0 = pr >= 0 && k < d.w, ok1 = pr >= 0 && k + 1 < d.w;
+      cp_async8_zfill(s, ok0 ? g : Pn, ok0 ? 8 : 0);
+      cp_async8_zfill(s + 1, ok1 ? g + 1 : Pn, ok1 ? 8 : 0);
+    }
+  }
+}
 
 __device__ __forceinline__ void wait_ge(const int* addr, int target) {
   int v;
@@ -331,27 +378,37 @@ __device__ __forceinline__ void wait_ge(const int* addr, int target) {
 __global__ void __launch_bounds__(CHOL_THREADS, 2) chol_col_kernel(CholArgs p) {
   extern __shared__ __align__(16) double smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  // Tile queue: the CTA draws a ticket when it starts RUNNING; ticket -> (block column j, row tile i, matrix b), ordered by
-  // column, the diagonal tile of a column first, the matrix index fastest.  A CTA only ever waits on tiles with a smaller
-  // ticket, and every smaller ticket was drawn by a CTA that is already running (or done): no deadlock whatever order the
-  // hardware dispatches blocks in (no reliance on in-order dispatch, MPS / preemption safe).
+  // Tile queue: the CTA draws a ticket when it starts RUNNING; ticket -> (group of matrices, block column j, row tile i, matrix b):
+  // the matrices in groups of p.group, one group after the other; inside a group ordered by column, the diagonal tile of a column
+  // first, the matrix index fastest.  A CTA only ever waits on tiles of its own matrix in earlier block columns, or on the diagonal
+  // tile of its own column: all in its group, with a smaller ticket.  Every smaller ticket was drawn by a CTA that is already running
+  // (or done): no deadlock whatever order the hardware dispatches blocks in (no reliance on in-order dispatch, MPS / preemption safe).
+  // (A group keeps the operands its later columns read -- the L tiles its earlier columns wrote -- in L2; one group of all B matrices
+  // sweeps the whole batch between a tile's write and its reads.)
   __shared__ int s_ticket;
   if (tid == 0) s_ticket = atomicAdd(p.ticket, 1);
   __syncthreads();
   const int64_t bid = s_ticket;
+  // block column j of one matrix starts at tile cs1(j) = j ntr - floor((j-1)^2 / 4) of that matrix (column j owns ntr - j/2 tiles)
+  auto cs1 = [&](int jj) -> int64_t { const int64_t m = jj > 0 ? jj - 1 : 0; return (int64_t)jj * p.ntr - (m * m) / 4; };
+  const int64_t per_group = cs1(p.nb) * p.group;
+  const int64_t g0 = (bid / per_group) * p.group;          // first matrix of the group
+  const int64_t gs = min((int64_t)p.group, p.B - g0);      // matrices in the group (the last one may be smaller)
+  const int64_t relg = bid - (g0 / p.group) * per_group;
   int j;
   {
-    int lo = 0, hi = p.nb;  // largest j with col_start[j] <= bid
+    int lo = 0, hi = p.nb;  // largest j with cs1(j) gs <= relg
     while (hi - lo > 1) {
       const int mid = (lo + hi) >> 1;
-      if (p.col_start[mid] <= bid) lo = mid; else hi = mid;
+      if (cs1(mid) * gs <= relg) lo = mid; else hi = mid;
     }
     j = lo;
   }
-  const int64_t rel = bid - p.col_start[j];
+  const int64_t rel = relg - cs1(j) * gs;
   const int i0 = j >> 1;                     // 128-row tile that contains the diagonal block of column j
-  const int64_t b = rel % p.B;
-  const int i = i0 + (int)(rel / p.B);
+  const int64_t b = g0 + rel % gs;
+  const int i = i0 + (int)(rel / gs);
+  const bool direct = p.d.fd != nullptr;
   const bool is_diag = (i == i0);
   const int roff = (j & 1) * 64;             // row offset of the diagonal block inside its tile
   const int64_t np = p.np;
@@ -365,7 +422,91 @@ __global__ void __launch_bounds__(CHOL_THREADS, 2) chol_col_kernel(CholArgs p) {
   // The accumulators start at -(AtA tile with the LM damping fused on the diagonal): the global loads are in flight
   // while the cp.async pipeline fills, and C = AtA - sum L L^T is simply -acc at the end (AtA is read exactly once).
   double acc[4][4][2];
-  {
+  double* Pn = nullptr;   // direct mode: this matrix's panel
+  if (direct) {
+    // Direct mode: the tile of the front matrix that front_assemble_kernel would have written -- zeros above the diagonal, identity on the
+    // padding, AtA (+ damping on the pivots' diagonal), then the children's update matrices added in list order -- gathered here: the same
+    // per-entry sums in the same order, so every value is bitwise the one it reads from the assembled matrix
+    const ThbCholDirect& d = p.d;
+    const int64_t* FD = d.fd;
+    Pn = d.factor + b * d.data_size + FD[4];
+    const double al = d.alpha != nullptr ? d.alpha[b] : 0.0;
+    const double be = d.beta != nullptr ? d.beta[b] : 0.0;
+    int li[4], lj[4][2];
+#pragma unroll
+    for (int mi = 0; mi < 4; mi++) li[mi] = direct_row(d, i * TM + wm * 32 + mi * 8 + lr);
+#pragma unroll
+    for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+      for (int u = 0; u < 2; u++) lj[ni][u] = direct_row(d, j * TN + wn * 32 + ni * 8 + lc * 2 + u);
+    // AtA: the panel-map entries of the 32 elements, then their values
+    int32_t m[4][4][2];
+#pragma unroll
+    for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+      for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+        for (int u = 0; u < 2; u++) {
+          const bool pan = li[mi] >= 0 && lj[ni][u] >= 0 && lj[ni][u] <= li[mi] && lj[ni][u] < d.w;
+          const int e = li[mi] * d.w + lj[ni][u];
+          m[mi][ni][u] = !pan ? -2 : (d.ata != nullptr ? __ldg(d.pmap + FD[4] + e) : e);
+        }
+#pragma unroll
+    for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+      for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+        for (int u = 0; u < 2; u++) {
+          const int gr = i * TM + wm * 32 + mi * 8 + lr, gc = j * TN + wn * 32 + ni * 8 + lc * 2 + u;
+          const int mm = m[mi][ni][u];
+          double x;
+          if (li[mi] < 0 || lj[ni][u] < 0) x = (gr == gc) ? 1.0 : 0.0;          // identity on the padding
+          else if (lj[ni][u] > li[mi] || mm == -1 || mm == -2) x = 0.0;          // above the diagonal; fill-in; border x border
+          else x = d.ata != nullptr ? __ldg(d.ata + b * d.ata_stride + mm) : Pn[mm];
+          if (mm != -2 && li[mi] == lj[ni][u]) x = x + (al * x + be);            // linear/utils.py:14-33: diag <- diag (1 + alpha) + beta
+          acc[mi][ni][u] = x;
+        }
+    // the children in list order, those whose rows reach the element; a child's inverse-map entries first, then its values
+    const int c_begin = (int)(FD[7] & 0xffffffffLL), nch = (int)(FD[7] >> 32);
+    for (int q = 0; q < nch; q++) {
+      const int64_t* PC = d.pc + (int64_t)(c_begin + q) * 6;   // (cb_off, cb_ld | b << 32, lo, hi, inv_off, u_off)
+      const double* src = d.arena_child + b * d.arena_size + PC[0];
+      const int ldg = (int)(PC[1] & 0xffffffffLL), lo = (int)PC[2], hi = (int)PC[3];
+      const int32_t* inv = d.c_inv + PC[4];
+      int ci[4], cj[4][2];
+#pragma unroll
+      for (int mi = 0; mi < 4; mi++) ci[mi] = (li[mi] >= lo && li[mi] <= hi) ? __ldg(inv + li[mi]) : -1;
+#pragma unroll
+      for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+        for (int u = 0; u < 2; u++) cj[ni][u] = (lj[ni][u] >= lo && lj[ni][u] <= hi) ? __ldg(inv + lj[ni][u]) : -1;
+#pragma unroll
+      for (int mi = 0; mi < 4; mi++) {
+        double x[4][2];
+#pragma unroll
+        for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+          for (int u = 0; u < 2; u++)
+            x[ni][u] = (ci[mi] >= 0 && cj[ni][u] >= 0 && lj[ni][u] <= li[mi]) ? __ldg(src + (int64_t)ci[mi] * ldg + cj[ni][u]) : -0.0;
+#pragma unroll
+        for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+          for (int u = 0; u < 2; u++) acc[mi][ni][u] = acc[mi][ni][u] + x[ni][u];
+      }
+    }
+    // the in-place form's read of the assembled value (no damping there: alpha, beta null)
+#pragma unroll
+    for (int mi = 0; mi < 4; mi++)
+#pragma unroll
+      for (int ni = 0; ni < 4; ni++)
+#pragma unroll
+        for (int u = 0; u < 2; u++) {
+          const int gr = i * TM + wm * 32 + mi * 8 + lr, gc = j * TN + wn * 32 + ni * 8 + lc * 2 + u;
+          double x = acc[mi][ni][u];
+          if (gr == gc) x = x + (0.0 * x + 0.0);
+          acc[mi][ni][u] = -x;
+        }
+  } else {
     const double* Ab = p.AtA + b * p.a_bstride;
     const double al = (p.alpha != nullptr) ? p.alpha[b] : 0.0;
     const double be = (p.beta != nullptr) ? p.beta[b] : 0.0;
@@ -404,13 +545,20 @@ __global__ void __launch_bounds__(CHOL_THREADS, 2) chol_col_kernel(CholArgs p) {
   const bool skip_mma = is_diag && (wm * 32 < roff);  // odd block columns: the upper 64 rows of the diagonal tile lie above the diagonal
   const double* Arow = Lb + (int64_t)i * TM * np;
   const double* Brow = Lb + (int64_t)j * TN * np;
+  auto load_stage = [&](int s, int k0) {
+    double* st = smem + (size_t)s * (A_TILE + B_TILE);
+    if (direct) {
+      load_panel_tile<TM>(st, Pn, p.d, i * TM, k0, tid);
+      if (!is_diag) load_panel_tile<TN>(st + A_TILE, Pn, p.d, j * TN, k0, tid);
+    } else {
+      load_oper_tile<TM, KB>(st, Arow, np, k0, tid);
+      if (!is_diag) load_oper_tile<TN, KB>(st + A_TILE, Brow, np, k0, tid);
+    }
+  };
   if (nk > 0) {
 #pragma unroll
     for (int s = 0; s < STAGES - 1; s++) {
-      if (s < nk) {
-        load_oper_tile<TM, KB>(smem + (size_t)s * (A_TILE + B_TILE), Arow, np, s * KB, tid);
-        if (!is_diag) load_oper_tile<TN, KB>(smem + (size_t)s * (A_TILE + B_TILE) + A_TILE, Brow, np, s * KB, tid);
-      }
+      if (s < nk) load_stage(s, s * KB);
       cp_async_commit();
     }
     for (int ks = 0; ks < nk; ks++) {
@@ -418,11 +566,7 @@ __global__ void __launch_bounds__(CHOL_THREADS, 2) chol_col_kernel(CholArgs p) {
       __syncthreads();
       {
         const int nx = ks + STAGES - 1;
-        if (nx < nk) {
-          const int s = nx % STAGES;
-          load_oper_tile<TM, KB>(smem + (size_t)s * (A_TILE + B_TILE), Arow, np, nx * KB, tid);
-          if (!is_diag) load_oper_tile<TN, KB>(smem + (size_t)s * (A_TILE + B_TILE) + A_TILE, Brow, np, nx * KB, tid);
-        }
+        if (nx < nk) load_stage(nx % STAGES, nx * KB);
         cp_async_commit();
       }
       const double* As = smem + (size_t)(ks % STAGES) * (A_TILE + B_TILE);
@@ -476,7 +620,18 @@ __global__ void __launch_bounds__(CHOL_THREADS, 2) chol_col_kernel(CholArgs p) {
 
   if (is_diag) {
     // ---------------- phase C: blocked potrf + triangular inverse of the 64x64 diagonal block ----------------
-    const int fail = diag64_factor_invert(Cs + roff * SC, smem + TM * SC, Lb + ((int64_t)j * TN) * np + (int64_t)j * TN, np, Wj);
+    int fail;
+    if (direct) {
+      // L_jj to the panel (its rows and columns below w), and the zeros of the panel above the diagonal in these rows
+      const int lim = min(TN, p.d.w - j * TN), c0 = (j + 1) * TN, nz = p.d.w - c0;
+      fail = diag64_factor_invert(Cs + roff * SC, smem + TM * SC, Pn + ((int64_t)j * TN) * p.d.w + (int64_t)j * TN, p.d.w, lim, Wj);
+      for (int e = tid; nz > 0 && e < lim * nz; e += CHOL_THREADS) {
+        const int rr = e / nz, c = e - rr * nz;
+        Pn[(int64_t)(j * TN + rr) * p.d.w + c0 + c] = 0.0;
+      }
+    } else {
+      fail = diag64_factor_invert(Cs + roff * SC, smem + TM * SC, Lb + ((int64_t)j * TN) * np + (int64_t)j * TN, np, TN, Wj);
+    }
     if (tid == 0 && fail != 0) record_first_failure(p.info + b, p.info_base + j * TN + fail);
     __threadfence();
     __syncthreads();
@@ -537,7 +692,21 @@ __global__ void __launch_bounds__(CHOL_THREADS, 2) chol_col_kernel(CholArgs p) {
     }
   }
   cp_async_wait<0>();
-  if (active) {
+  if (active && direct) {
+#pragma unroll
+    for (int mi = 0; mi < 2; mi++) {
+      const int pr = direct_row(p.d, i * TM + warp * 16 + mi * 8 + lr);
+      if (pr < 0) continue;
+      double* dst = Pn + (int64_t)pr * p.d.w;
+#pragma unroll
+      for (int ni = 0; ni < 8; ni++)
+#pragma unroll
+        for (int u = 0; u < 2; u++) {
+          const int c = j * TN + ni * 8 + lc * 2 + u;
+          if (c < p.d.w) dst[c] = acc2[mi][ni][u];
+        }
+    }
+  } else if (active) {
 #pragma unroll
     for (int mi = 0; mi < 2; mi++) {
       const int r = warp * 16 + mi * 8 + lr;
@@ -682,7 +851,6 @@ struct Geometry {
   int* flags;
   int* done;
   int* ticket;
-  int64_t* col_start;
 };
 static inline Geometry geometry(void* workspace, int64_t B, int64_t n) {
   Geometry g;
@@ -694,18 +862,16 @@ static inline Geometry geometry(void* workspace, int64_t B, int64_t n) {
   g.flags = reinterpret_cast<int*>(g.W + B * g.nb * TN * TN);
   g.done = g.flags + align_up(B * g.nb, 64);
   g.ticket = g.done + align_up(B * g.ntr, 64);
-  g.col_start = reinterpret_cast<int64_t*>(g.ticket + 64);
   return g;
 }
 
-// First CTA index of every block column: column j owns (ntr - j/2) * B CTAs, so col_start[j] = B * (j*ntr - floor((j-1)^2/4)).
-// Filled on the device (not copied from a host array): the entry point must be capturable into a CUDA graph, and a captured H2D
-// copy would re-read a dead stack address at every replay.
-__global__ void chol_col_start_kernel(int64_t* __restrict__ col_start, int nb, int ntr, int64_t B) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j > nb) return;
-  const int64_t jm1 = j > 0 ? j - 1 : 0;
-  col_start[j] = B * ((int64_t)j * ntr - (jm1 * jm1) / 4);
+// Partial mode: tickets in groups of this many matrices (THB_CHOL_GROUP, read at every call; 0 or unset: the default below, which is
+// clamped to B)
+static inline int64_t chol_partial_group(int64_t B) {
+  const char* e = getenv("THB_CHOL_GROUP");
+  int64_t g = e != nullptr ? atoll(e) : 0;
+  if (g <= 0) g = THB_CHOL_GROUP_DEFAULT;
+  return g < B ? g : B;
 }
 
 }  // namespace thb
@@ -720,7 +886,6 @@ int64_t thb_potrf_workspace_bytes(int64_t B, int64_t n) {
   bytes += thb::align_up(B * nb, 64) * 4;                       // flags (W_j ready)
   bytes += thb::align_up(B * (np / thb::TM), 64) * 4;           // finished-column counters per row tile
   bytes += 64 * 4;                                              // tile-queue ticket counter
-  bytes += (nb + 1) * 8;                                        // first CTA index of every block column
   return thb::align_up(bytes, 256);
 }
 
@@ -733,28 +898,25 @@ int thb_potrf_f64(const double* AtA, const double* alpha, const double* beta, in
   thb::Geometry g = thb::geometry(workspace, B, n);
   THB_CUDA(cudaMemsetAsync(g.flags, 0, (size_t)(thb::align_up(B * g.nb, 64) + thb::align_up(B * g.ntr, 64) + 64) * 4, cs));  // flags, done, ticket
   THB_CUDA(cudaMemsetAsync(info, 0, (size_t)B * 4, cs));
-  // CTA index table (host-computed, tiny): column j owns (ntr - j/2) * B CTAs
-  int64_t starts[1026];
+  // CTAs: column j owns (ntr - j/2) * B
   if (g.nb > 1024) return THB_ERR_UNSUPPORTED;
-  starts[0] = 0;
-  for (int j = 0; j < g.nb; j++) starts[j + 1] = starts[j] + (int64_t)(g.ntr - (j >> 1)) * B;
-  if (starts[g.nb] > 2147483647LL) return THB_ERR_UNSUPPORTED;
-  thb::chol_col_start_kernel<<<(unsigned)((g.nb + 1 + 255) / 256), 256, 0, cs>>>(g.col_start, (int)g.nb, (int)g.ntr, B);
-  THB_CHECK_LAUNCH();
+  int64_t total = 0;
+  for (int j = 0; j < g.nb; j++) total += (int64_t)(g.ntr - (j >> 1)) * B;
+  if (total > 2147483647LL) return THB_ERR_UNSUPPORTED;
   static bool attr_set = false;
   if (!attr_set) {
     THB_CUDA(cudaFuncSetAttribute(thb::chol_col_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)thb::CHOL_SMEM));
     attr_set = true;
   }
   thb::CholArgs a;
-  a.AtA = AtA; a.alpha = alpha; a.beta = beta; a.L = g.L; a.W = g.W; a.flags = g.flags; a.done = g.done;
-  a.col_start = g.col_start; a.info = info;
+  a.AtA = AtA; a.alpha = alpha; a.beta = beta; a.L = g.L; a.W = g.W; a.flags = g.flags; a.done = g.done; a.info = info;
   a.B = B; a.n = n; a.np = g.np; a.nb = g.nb; a.ntr = g.ntr;
   a.ticket = g.ticket; a.nb_piv = g.nb; a.a_bstride = n * n; a.l_bstride = g.np * g.np; a.info_base = 0;
   a.k_lim = g.nb * (thb::TN / thb::KB); a.n_real = (int)g.np;
+  a.group = (int)B; a.d = ThbCholDirect{};   // the whole batch is one group
   // ONE launch for the whole factorisation: block columns are chained through the per-tile counters, so there are
   // no per-column launch gaps and no per-column wave-quantisation tails.
-  thb::chol_col_kernel<<<(unsigned)starts[g.nb], thb::CHOL_THREADS, thb::CHOL_SMEM, cs>>>(a);
+  thb::chol_col_kernel<<<(unsigned)total, thb::CHOL_THREADS, thb::CHOL_SMEM, cs>>>(a);
   THB_CHECK_LAUNCH();
   return THB_OK;
 }
@@ -788,12 +950,12 @@ int64_t thb_potrf_partial_workspace_bytes(int64_t B, int64_t np) {
   if (B <= 0 || np <= 0) return 0;
   const int64_t nb = np / thb::TN;
   int64_t bytes = B * nb * thb::TN * thb::TN * 8;               // W
-  bytes += thb::align_up(B * nb, 64) * 4 + thb::align_up(B * (np / thb::TM), 64) * 4 + 64 * 4 + (nb + 1) * 8;
+  bytes += thb::align_up(B * nb, 64) * 4 + thb::align_up(B * (np / thb::TM), 64) * 4 + 64 * 4;
   return thb::align_up(bytes, 256);
 }
 
-int thb_potrf_partial_inplace_f64(double* F, int64_t bstride, int64_t np, int32_t nb_piv, int32_t w_real, int32_t n_real, int32_t info_base,
-                                  int32_t* info, int64_t B, void* workspace, int64_t workspace_bytes, thb_stream_t stream) {
+static int potrf_partial(double* F, int64_t bstride, int64_t np, int32_t nb_piv, int32_t w_real, int32_t n_real, int32_t info_base,
+                         int32_t* info, int64_t B, void* workspace, int64_t workspace_bytes, const ThbCholDirect* direct, thb_stream_t stream) {
   if (B < 0 || np <= 0 || np % thb::TM != 0 || F == nullptr || info == nullptr || workspace == nullptr) return THB_ERR_BAD_ARG;
   if (B == 0) return THB_OK;
   if (workspace_bytes < thb_potrf_partial_workspace_bytes(B, np)) return THB_ERR_BAD_ARG;
@@ -804,27 +966,46 @@ int thb_potrf_partial_inplace_f64(double* F, int64_t bstride, int64_t np, int32_
   int* flags = reinterpret_cast<int*>(W + B * nb * thb::TN * thb::TN);
   int* done = flags + thb::align_up(B * nb, 64);
   int* ticket = done + thb::align_up(B * ntr, 64);
-  int64_t* col_start = reinterpret_cast<int64_t*>(ticket + 64);
   THB_CUDA(cudaMemsetAsync(flags, 0, (size_t)(thb::align_up(B * nb, 64) + thb::align_up(B * ntr, 64) + 64) * 4, cs));
   int64_t total = 0;
   for (int j = 0; j < nb; j++) total += (int64_t)(ntr - (j >> 1)) * B;
   if (total > 2147483647LL) return THB_ERR_UNSUPPORTED;
-  thb::chol_col_start_kernel<<<(unsigned)((nb + 1 + 255) / 256), 256, 0, cs>>>(col_start, nb, ntr, B);
-  THB_CHECK_LAUNCH();
   static bool attr_set = false;
   if (!attr_set) {
     THB_CUDA(cudaFuncSetAttribute(thb::chol_col_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)thb::CHOL_SMEM));
     attr_set = true;
   }
   thb::CholArgs a;
-  a.AtA = F; a.alpha = nullptr; a.beta = nullptr; a.L = F; a.W = W; a.flags = flags; a.done = done; a.col_start = col_start; a.info = info;
+  a.AtA = F; a.alpha = nullptr; a.beta = nullptr; a.L = F; a.W = W; a.flags = flags; a.done = done; a.info = info;
   a.B = B; a.n = np; a.np = np; a.nb = nb; a.ntr = ntr;
   a.ticket = ticket; a.nb_piv = nb_piv; a.a_bstride = bstride; a.l_bstride = bstride; a.info_base = info_base;
   a.k_lim = (w_real > 0 && nb_piv < nb) ? (w_real + thb::KB - 1) / thb::KB : nb * (thb::TN / thb::KB);
   a.n_real = (n_real > 0 && n_real <= np) ? n_real : (int)np;
+  a.group = (int)thb::chol_partial_group(B);
+  a.d = direct != nullptr ? *direct : ThbCholDirect{};
   thb::chol_col_kernel<<<(unsigned)total, thb::CHOL_THREADS, thb::CHOL_SMEM, cs>>>(a);
   THB_CHECK_LAUNCH();
   return THB_OK;
+}
+
+/* Partial in-place factorisation of B frontal matrices (multifrontal block-sparse Cholesky, thb_front.cu): F_b = F + b * bstride is an
+ * np x np row-major matrix (np a multiple of 128; lower part + diagonal tiles read).  The first nb_piv 64-wide block columns are
+ * factored (L in place, zeros above the diagonal of the diagonal blocks), the trailing (np - 64 nb_piv)^2 block becomes the Schur
+ * complement F22 - L21 L21^T in place.  w_real (> 0): number of real pivot columns -- the identity padding of the last pivot block column is
+ * skipped by the k loops; n_real (> 0): rows / columns from n_real on are padding -- trailing tiles entirely there are skipped.
+ * info[b] (NOT cleared here) receives info_base + 1 + index of the first non-positive pivot. */
+int thb_potrf_partial_inplace_f64(double* F, int64_t bstride, int64_t np, int32_t nb_piv, int32_t w_real, int32_t n_real, int32_t info_base,
+                                  int32_t* info, int64_t B, void* workspace, int64_t workspace_bytes, thb_stream_t stream) {
+  return potrf_partial(F, bstride, np, nb_piv, w_real, n_real, info_base, info, B, workspace, workspace_bytes, nullptr, stream);
+}
+
+/* The same factorisation of a big front of the multifrontal factor without the assembled matrix: its tiles are gathered from AtA and the
+ * children's update matrices (direct->fd), the pivot columns' L goes to the front's panel (row-major (w + b) x w in the factor storage,
+ * zeros above the diagonal) and is read back from there; only the trailing block -- the update matrix -- is written to F. */
+int thb_potrf_partial_direct_f64(double* F, int64_t bstride, int64_t np, int32_t nb_piv, int32_t n_real, int32_t info_base, int32_t* info,
+                                 int64_t B, void* workspace, int64_t workspace_bytes, const ThbCholDirect* direct, thb_stream_t stream) {
+  if (direct == nullptr || direct->fd == nullptr || direct->w <= 0 || direct->wpad != nb_piv * thb::TN) return THB_ERR_BAD_ARG;
+  return potrf_partial(F, bstride, np, nb_piv, direct->w, n_real, info_base, info, B, workspace, workspace_bytes, direct, stream);
 }
 
 #ifdef THB_CHOL_TIMING

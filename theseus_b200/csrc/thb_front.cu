@@ -10,9 +10,9 @@
 // Small fronts (r <= 160): ONE CTA per (front, item), the whole front in shared memory: scatter-add of the children, scalar
 //   right-looking pivots on the r x w panel, the rank-w update of C on the FP64 tensor pipe (mma.sync m8n8k4 DMMA, 16x16 macro
 //   tiles per warp) -- every byte of a small front is read once and written once.
-// Big fronts: assembled into a padded dense matrix in global memory (row tiles in shared memory, children added in a fixed order),
-//   then the DMMA dense kernel of thb_chol_dense.cu in partial mode (left-looking tiles: the Schur complement is accumulated in
-//   registers over all pivot columns and written once), then the panel is copied to the factor storage.
+// Big fronts: the DMMA dense kernel of thb_chol_dense.cu in partial mode (left-looking tiles: the Schur complement is accumulated in
+//   registers over all pivot columns and written once), each tile gathered from AtA and the children (in a fixed order), L stored
+//   straight into the panel in the factor storage.
 // Substitutions: per front one CTA per item, chunked by 32 pivot columns: a 32 x 32 triangular block is solved by one warp with
 //   shuffles, the rest of the panel is a row-contiguous mat-vec; the forward pass hands border vectors to the parent through a
 //   second ping-pong arena, the backward pass gathers the ancestors' solution.  The permutation is folded into the first load /
@@ -998,6 +998,14 @@ __global__ void __launch_bounds__(THREADS) front_backward_kernel(FrontSolveArgs 
   }
 }
 
+// Big fronts: factored by the dense kernel straight into their panel (default), or -- THB_FRONT_BIG_DIRECT=0, read at every call: the
+// reference the tests compare the direct form against -- assembled into the padded front matrix (front_assemble_kernel), factored in
+// place and copied out (front_extract_kernel)
+static inline bool front_big_direct() {
+  const char* e = getenv("THB_FRONT_BIG_DIRECT");
+  return !(e != nullptr && e[0] == '0');
+}
+
 static inline int front_threads_of_class(int cls) { return cls == 0 ? 64 : (cls == 1 ? 128 : 256); }
 
 // Opt in to the launch's dynamic shared memory whenever it grows, not only above 48 KB: the 48 KB default limit also counts the kernel's
@@ -1053,7 +1061,7 @@ static int front_solve_launch(const thb_front_plan* p, const int64_t* L, int pas
 }
 
 // The numeric factorisation; with rhs != null also the forward substitution: fused into front_small_kernel for the shared-memory
-// fronts, front_forward_kernel right after the extraction of a big front's panel.
+// fronts, front_forward_kernel right after the dense kernel has written a big front's panel.
 static int front_factor(const thb_front_plan* p, const int64_t* launches, int64_t num_launches, double* factor, const double* ata,
                         int64_t ata_stride, const double* alpha, const double* beta, double* arena, void* dense_ws, int64_t dense_ws_bytes,
                         int32_t* info, const double* rhs, double* work, double* varena, int64_t B, thb_stream_t stream) {
@@ -1128,12 +1136,30 @@ static int front_factor(const thb_front_plan* p, const int64_t* launches, int64_
       return THB_ERR_UNSUPPORTED;   // the DMMA dense kernel is not part of the host emulation
 #else
       if (dense_ws == nullptr || np % 128 != 0 || np > 8192) return THB_ERR_BAD_ARG;
+      const int32_t n_real = (int32_t)(nb_piv * 64 + L[11]);
+      if (front_big_direct()) {
+        // the dense kernel gathers the front's tiles from AtA and the children, and factors straight into the front's panel
+        ThbCholDirect d;
+        d.fd = p->fd + (int64_t)begin * 8; d.pc = p->pc; d.c_inv = p->c_inv; d.pmap = p->pmap;
+        d.factor = factor; d.data_size = p->data_size;
+        d.arena_child = a.arena_child; d.arena_size = p->arena_size;
+        d.ata = a.ata; d.ata_stride = ata_stride; d.alpha = alpha; d.beta = beta;
+        d.w = (int)L[10]; d.b = (int)L[11]; d.wpad = (int)(nb_piv * 64);
+        int rc = thb_potrf_partial_direct_f64(a.arena_cur + fr_off, p->arena_size, np, (int32_t)nb_piv, n_real, (int32_t)first, info, B,
+                                              dense_ws, dense_ws_bytes, &d, stream);
+        if (rc != THB_OK) return rc;
+        if (rhs != nullptr) {
+          rc = front_solve_launch(p, L, 0, factor, rhs, nullptr, work, varena, B, cs);
+          if (rc != THB_OK) return rc;
+        }
+        continue;
+      }
       const size_t smem = (size_t)ASM_ROWS * np * 8;
       int rc = front_set_smem(front_assemble_kernel, smem, &asm_set); if (rc) return rc;
       front_assemble_kernel<<<dim3((unsigned)B, (unsigned)(np / ASM_ROWS)), ASM_THREADS, smem, cs>>>(a, t);
       THB_CHECK_LAUNCH();
       // w_real / n_real: the k loops stop at the real pivot columns, trailing tiles that lie in the padding are skipped
-      rc = thb_potrf_partial_inplace_f64(a.arena_cur + fr_off, p->arena_size, np, (int32_t)nb_piv, (int32_t)L[10], (int32_t)(nb_piv * 64 + L[11]),
+      rc = thb_potrf_partial_inplace_f64(a.arena_cur + fr_off, p->arena_size, np, (int32_t)nb_piv, (int32_t)L[10], n_real,
                                          (int32_t)first, info, B, dense_ws, dense_ws_bytes, stream);
       if (rc != THB_OK) return rc;
       front_extract_kernel<<<dim3((unsigned)B, 8), 256, 0, cs>>>(a, t);
