@@ -1,4 +1,4 @@
-"""The fused motion-planning and planar-pushing kernels (linearize_mp_kernel / error_mp_kernel: Collision2D on Point2 / SE2,
+"""The fused motion-planning and planar-pushing kernels (linearize_kernel / error_kernel over MpCost: Collision2D on Point2 / SE2,
 DoubleIntegrator on Vector (D = 1, 2, 3) / SE2 with Scale, Diagonal or GP weights, HingeCost (D = 1, 2, 3), Nonholonomic on SE2 / Vector,
 QuasiStaticPushingPlanar, EffectorObjectContactPlanar) compared entry by entry with the float64 restatement of oracle/embodied.py, through
 the public API (th.eb.*) and the engine's linearize_sparse / error_metric:

@@ -261,82 +261,6 @@ __device__ __forceinline__ void se2_cost(const GroupDev<T>& g, int k, int64_t b,
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-template <typename T, int KIND>
-__global__ void __launch_bounds__(128) linearize_kernel(GroupDev<T> g, int64_t B, T* __restrict__ A_val, int64_t nnz,
-                                                        T* __restrict__ bvec, int64_t m) {
-  extern __shared__ double lin_stage_raw[];
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const bool valid = t < (int64_t)g.K * B;     // (no early exit: every lane takes part in the warp-cooperative store below)
-  const int k = valid ? (int)(t / B) : 0;
-  const int64_t b = valid ? t - (int64_t)k * B : 0;
-  constexpr int DIM = (KIND == THB_COST_BETWEEN_SE3 || KIND == THB_COST_LOCAL_SE3) ? 6 : 3;
-  constexpr bool BETWEEN = (KIND == THB_COST_BETWEEN_SE3 || KIND == THB_COST_BETWEEN_SO3 || KIND == THB_COST_BETWEEN_SE2);
-  constexpr bool IS_SE2 = (KIND == THB_COST_BETWEEN_SE2 || KIND == THB_COST_LOCAL_SE2);
-  T w[DIM], e[DIM], J0[DIM * DIM], J1[DIM * DIM];
-  const bool masked = load_weight<T, DIM>(g, k, b, w);
-  if (masked) {
-#pragma unroll
-    for (int i = 0; i < DIM; i++) e[i] = T(0);
-#pragma unroll
-    for (int i = 0; i < DIM * DIM; i++) { J0[i] = T(0); J1[i] = T(0); }
-  } else if (DIM == 6) {
-    se3_cost<T, true, BETWEEN>(g, k, b, w, e, J0, J1);
-  } else if (IS_SE2) {
-    se2_cost<T, true, BETWEEN>(g, k, b, w, e, J0, J1);
-  } else {
-    so3_cost<T, true, BETWEEN>(g, k, b, w, e, J0, J1);
-  }
-  if (g.robust_kind != THB_ROBUST_NONE && !masked) {
-    T x = T(0);
-#pragma unroll
-    for (int r = 0; r < DIM; r++) x += e[r] * e[r];
-    const T sc = robust_rescale(g, k, b, x);
-#pragma unroll
-    for (int r = 0; r < DIM; r++) e[r] *= sc;
-#pragma unroll
-    for (int i = 0; i < DIM * DIM; i++) { J0[i] *= sc; if (BETWEEN) J1[i] *= sc; }
-  }
-  // A cost function's rows of A_val are ONE contiguous run of DIM * stride values per batch item (stride = its row length), but the
-  // items of a warp lie nnz values apart: storing from the computing thread writes 8 bytes to 32 different sectors per instruction.
-  // Stage the warp's 32 runs in shared memory and let the whole warp store each run with consecutive lanes (256-byte segments).
-  T* Arow = A_val + b * nnz + g.a_off[k];
-  const int stride = g.a_stride[k];
-  constexpr int NVMAX = DIM * DIM * (BETWEEN ? 2 : 1);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  T* stage = reinterpret_cast<T*>(lin_stage_raw) + (size_t)warp * 32 * (NVMAX + 1);
-  T* mine = stage + lane * (NVMAX + 1);
-  const int nv = DIM * stride;                 // <= NVMAX by construction of the groups (stride = DIM or 2 DIM)
-  const int bp0 = g.bp[k * 2 + 0];
-#pragma unroll
-  for (int r = 0; r < DIM; r++)
-#pragma unroll
-    for (int c = 0; c < DIM; c++) mine[r * stride + bp0 + c] = J0[r * DIM + c];
-  if (BETWEEN) {
-    const int bp1 = g.bp[k * 2 + 1];
-#pragma unroll
-    for (int r = 0; r < DIM; r++)
-#pragma unroll
-      for (int c = 0; c < DIM; c++) mine[r * stride + bp1 + c] = J1[r * DIM + c];
-  }
-  __syncwarp();
-  const unsigned long long my_dst = valid ? reinterpret_cast<unsigned long long>(Arow) : 0ull;
-  for (int i = 0; i < 32; i++) {
-    const unsigned long long d = __shfl_sync(0xffffffffu, my_dst, i);
-    const int nvi = __shfl_sync(0xffffffffu, nv, i);
-    if (d != 0ull) {
-      T* dst = reinterpret_cast<T*>(d);
-      const T* src = stage + i * (NVMAX + 1);
-      for (int v = lane; v < nvi; v += 32) dst[v] = src[v];
-    }
-  }
-  if (valid) {
-    T* brow = bvec + b * m + g.row0[k];
-#pragma unroll
-    for (int r = 0; r < DIM; r++) brow[r] = -e[r];
-  }
-}
-
 // Reprojection (theseus/embodied/measurements/reprojection.py:54-94): q = R p + t, proj = -q_xy/q_z,
 // e = proj * f (1 + n (k1 + n k2)) - z with n = |proj|^2.  Jacobians by the quotient rule on
 // [R, -R hat(p) | R] (torchlie se3_impl.py:764-777), exactly as the reference composes them.
@@ -386,67 +310,6 @@ __device__ __forceinline__ void reprojection_cost(const GroupDev<T>& g, int k, i
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(128) linearize_reprojection_kernel(GroupDev<T> g, int64_t B, T* __restrict__ A_val, int64_t nnz,
-                                                                     T* __restrict__ bvec, int64_t m) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= (int64_t)g.K * B) return;
-  const int k = (int)(t / B);
-  const int64_t b = t - (int64_t)k * B;
-  T w[2], e[2], Jc[12], Jp[6];
-  const bool masked = load_weight<T, 2>(g, k, b, w);
-  if (masked) {
-    e[0] = e[1] = T(0);
-#pragma unroll
-    for (int i = 0; i < 12; i++) Jc[i] = T(0);
-#pragma unroll
-    for (int i = 0; i < 6; i++) Jp[i] = T(0);
-  } else {
-    reprojection_cost<T, true>(g, k, b, w, e, Jc, Jp);
-    if (g.robust_kind != THB_ROBUST_NONE) {
-      const T sc = robust_rescale(g, k, b, e[0] * e[0] + e[1] * e[1]);
-      e[0] *= sc;
-      e[1] *= sc;
-#pragma unroll
-      for (int i = 0; i < 12; i++) Jc[i] *= sc;
-#pragma unroll
-      for (int i = 0; i < 6; i++) Jp[i] *= sc;
-    }
-  }
-  T* Arow = A_val + b * nnz + g.a_off[k];
-  const int stride = g.a_stride[k];
-  const int bp0 = g.bp[k * 2 + 0], bp1 = g.bp[k * 2 + 1];
-#pragma unroll
-  for (int r = 0; r < 2; r++) {
-#pragma unroll
-    for (int c = 0; c < 6; c++) Arow[r * stride + bp0 + c] = Jc[r * 6 + c];
-#pragma unroll
-    for (int c = 0; c < 3; c++) Arow[r * stride + bp1 + c] = Jp[r * 3 + c];
-  }
-  T* brow = bvec + b * m + g.row0[k];
-  brow[0] = -e[0];
-  brow[1] = -e[1];
-}
-
-template <typename T>
-__global__ void __launch_bounds__(128) error_reprojection_kernel(GroupDev<T> g, int64_t B, T* __restrict__ partial) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int nchunks = (g.K + kErrCostsPerThread - 1) / kErrCostsPerThread;
-  if (t >= (int64_t)nchunks * B) return;
-  const int c = (int)(t / B);
-  const int64_t b = t - (int64_t)c * B;
-  T acc = T(0);
-  const int k1 = min(g.K, (c + 1) * kErrCostsPerThread);
-  for (int k = c * kErrCostsPerThread; k < k1; k++) {
-    T w[2], e[2];
-    if (load_weight<T, 2>(g, k, b, w)) continue;
-    reprojection_cost<T, false>(g, k, b, w, e, nullptr, nullptr);
-    const T x = e[0] * e[0] + e[1] * e[1];
-    acc += (g.robust_kind != THB_ROBUST_NONE) ? robust_value(g, k, b, x, 2) : x;
-  }
-  partial[(int64_t)c * B + b] = acc * T(0.5);
-}
-
 // Difference on Vector/Point: e = (x - target) * w ; J = I * w   (geometry/vector.py local/jacobians)
 // true if every weight of this (k, b) is zero: the cost function is masked like the other kinds (load_weight), its x / target not read
 template <typename T> __device__ __forceinline__ bool vector_masked(const GroupDev<T>& g, const T* wp) {
@@ -455,84 +318,13 @@ template <typename T> __device__ __forceinline__ bool vector_masked(const GroupD
     if (wp[r] != T(0)) return false;
   return true;
 }
-template <typename T>
-__global__ void linearize_vector_kernel(GroupDev<T> g, int64_t B, T* __restrict__ A_val, int64_t nnz,
-                                        T* __restrict__ bvec, int64_t m) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= (int64_t)g.K * B) return;
-  const int k = (int)(t / B);
-  const int64_t b = t - (int64_t)k * B;
-  const int d = g.dim;
-  const T* x = g.x0[k] + (int64_t)g.bstride[k * 4 + 0] * b;
-  const T* tg = g.aux[k] + (int64_t)g.bstride[k * 4 + 2] * b;
-  const T* wp = g.w[k] + (int64_t)g.bstride[k * 4 + 3] * b;
-  T* Arow = A_val + b * nnz + g.a_off[k];
-  const int stride = g.a_stride[k];
-  const int bp0 = g.bp[k * 2 + 0];
-  T* brow = bvec + b * m + g.row0[k];
-  const bool masked = vector_masked(g, wp);
-  for (int r = 0; r < d; r++) {
-    const T w = masked ? T(0) : ((g.weight_kind == THB_WEIGHT_SCALE) ? wp[0] : wp[r]);
-    for (int c = 0; c < d; c++) Arow[r * stride + bp0 + c] = (r == c) ? w : T(0);
-    brow[r] = masked ? T(0) : -((x[r] - tg[r]) * w);
-  }
-}
-
-template <typename T, int KIND>
-__global__ void __launch_bounds__(128) error_kernel(GroupDev<T> g, int64_t B, T* __restrict__ partial) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int nchunks = (g.K + kErrCostsPerThread - 1) / kErrCostsPerThread;
-  if (t >= (int64_t)nchunks * B) return;
-  const int c = (int)(t / B);
-  const int64_t b = t - (int64_t)c * B;
-  constexpr int DIM = (KIND == THB_COST_BETWEEN_SE3 || KIND == THB_COST_LOCAL_SE3) ? 6 : 3;
-  constexpr bool BETWEEN = (KIND == THB_COST_BETWEEN_SE3 || KIND == THB_COST_BETWEEN_SO3 || KIND == THB_COST_BETWEEN_SE2);
-  constexpr bool IS_SE2 = (KIND == THB_COST_BETWEEN_SE2 || KIND == THB_COST_LOCAL_SE2);
-  T acc = T(0);
-  const int k1 = min(g.K, (c + 1) * kErrCostsPerThread);
-  for (int k = c * kErrCostsPerThread; k < k1; k++) {
-    T w[DIM], e[DIM];
-    const bool masked = load_weight<T, DIM>(g, k, b, w);
-    if (masked) continue;
-    if (DIM == 6) se3_cost<T, false, BETWEEN>(g, k, b, w, e, nullptr, nullptr);
-    else if (IS_SE2) se2_cost<T, false, BETWEEN>(g, k, b, w, e, nullptr, nullptr);
-    else so3_cost<T, false, BETWEEN>(g, k, b, w, e, nullptr, nullptr);
-    T x = T(0);
-#pragma unroll
-    for (int r = 0; r < DIM; r++) x += e[r] * e[r];
-    acc += (g.robust_kind != THB_ROBUST_NONE) ? robust_value(g, k, b, x, DIM) : x;
-  }
-  partial[(int64_t)c * B + b] = acc * T(0.5);
-}
-
-template <typename T> __global__ void error_vector_kernel(GroupDev<T> g, int64_t B, T* __restrict__ partial) {
-  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int nchunks = (g.K + kErrCostsPerThread - 1) / kErrCostsPerThread;
-  if (t >= (int64_t)nchunks * B) return;
-  const int c = (int)(t / B);
-  const int64_t b = t - (int64_t)c * B;
-  T acc = T(0);
-  const int k1 = min(g.K, (c + 1) * kErrCostsPerThread);
-  for (int k = c * kErrCostsPerThread; k < k1; k++) {
-    const T* x = g.x0[k] + (int64_t)g.bstride[k * 4 + 0] * b;
-    const T* tg = g.aux[k] + (int64_t)g.bstride[k * 4 + 2] * b;
-    const T* wp = g.w[k] + (int64_t)g.bstride[k * 4 + 3] * b;
-    if (vector_masked(g, wp)) continue;
-    for (int r = 0; r < g.dim; r++) {
-      const T w = (g.weight_kind == THB_WEIGHT_SCALE) ? wp[0] : wp[r];
-      const T e = (x[r] - tg[r]) * w;
-      acc += e * e;
-    }
-  }
-  partial[(int64_t)c * B + b] = acc * T(0.5);
-}
 
 // ------------------------------------------------------------------------------------------------
 // Motion-planning cost functions: Collision2D (embodied/collision/collision.py:44-73 + signed_distance_field.py:163-241),
 // DoubleIntegrator / GPMotionModel (motionmodel/double_integrator.py:45-80) with GPCostWeight (:131-170), HingeCost and
 // Nonholonomic (motionmodel/misc.py:62-84, 126-178).  Every optimisation variable of one of these cost functions has the same dof D;
 // a cost function's row block is DIM x (NVARS * D).  The unweighted Jacobian is written straight into the warp's staging area (the
-// layout of A_val), the weight is applied there, and the warp stores the rows with consecutive lanes like linearize_kernel.
+// layout of A_val) and the weight is applied there.
 template <typename T> __device__ __forceinline__ T t_floor(T x);
 template <> __device__ __forceinline__ float t_floor<float>(float x) { return floorf(x); }
 template <> __device__ __forceinline__ double t_floor<double>(double x) { return floor(x); }
@@ -850,55 +642,219 @@ template <typename T, int DIM, int D> struct MpWeight {
   }
 };
 
-template <typename T, int KIND, int D>
-__global__ void __launch_bounds__(128) linearize_mp_kernel(GroupDev<T> g, int64_t B, T* __restrict__ A_val, int64_t nnz,
-                                                           T* __restrict__ bvec, int64_t m) {
+// ------------------------------------------------------------------------------------------------
+// One policy per cost family for linearize_kernel / error_kernel.  A policy gives
+//   DIM      rows of a cost function (VectorCost: 0, its g.dim rows are known at run time only)
+//   NV       values of its row block staged per thread for the warp-cooperative store (0: each thread stores its own rows)
+//   ROBUST   whether the group's robust loss applies (RobustCostFunction routes the Lie and Reprojection kinds only)
+//   load(g, k, b)                the weights of (k, b); true if they are all zero (masked cost function: nothing else is read)
+//   linearize(g, k, b, e, row)   the weighted error e and weighted Jacobian rows, written to row (row-major, A_val layout).  ROBUST
+//                                policies keep their Jacobians in J instead, so that the robust rescale happens in registers, and
+//                                write them with store(g, k, row)
+//   error(g, k, b, acc)          adds the cost function's share of the error metric to acc (after load)
+template <int N, typename T> __device__ __forceinline__ T sum_sq(const T* e) {
+  T x = T(0);
+#pragma unroll
+  for (int r = 0; r < N; r++) x += e[r] * e[r];
+  return x;
+}
+
+template <typename T, int KIND> struct LieCost {
+  static constexpr int DIM = (KIND == THB_COST_BETWEEN_SE3 || KIND == THB_COST_LOCAL_SE3) ? 6 : 3;
+  static constexpr bool BETWEEN = (KIND == THB_COST_BETWEEN_SE3 || KIND == THB_COST_BETWEEN_SO3 || KIND == THB_COST_BETWEEN_SE2);
+  static constexpr bool IS_SE2 = (KIND == THB_COST_BETWEEN_SE2 || KIND == THB_COST_LOCAL_SE2);
+  static constexpr int NV = DIM * DIM * (BETWEEN ? 2 : 1), NJ = NV;
+  static constexpr bool ROBUST = true;
+  T w[DIM], J[NJ];   // J0, then (Between) J1
+
+  __device__ __forceinline__ bool load(const GroupDev<T>& g, int k, int64_t b) { return load_weight<T, DIM>(g, k, b, w); }
+  template <bool WITH_J> __device__ __forceinline__ void cost(const GroupDev<T>& g, int k, int64_t b, T* e) {
+    if (DIM == 6) se3_cost<T, WITH_J, BETWEEN>(g, k, b, w, e, J, J + DIM * DIM);
+    else if (IS_SE2) se2_cost<T, WITH_J, BETWEEN>(g, k, b, w, e, J, J + DIM * DIM);
+    else so3_cost<T, WITH_J, BETWEEN>(g, k, b, w, e, J, J + DIM * DIM);
+  }
+  __device__ __forceinline__ void linearize(const GroupDev<T>& g, int k, int64_t b, T* e, T*) { cost<true>(g, k, b, e); }
+  static __device__ __forceinline__ T sqnorm(const T* e) { return sum_sq<DIM>(e); }
+  __device__ __forceinline__ void store(const GroupDev<T>& g, int k, T* row) const {
+    const int stride = g.a_stride[k];
+    const int bp0 = g.bp[k * 2 + 0];
+#pragma unroll
+    for (int r = 0; r < DIM; r++)
+#pragma unroll
+      for (int c = 0; c < DIM; c++) row[r * stride + bp0 + c] = J[r * DIM + c];
+    if (BETWEEN) {   // after J0: J1 wins where bp0 == bp1
+      const int bp1 = g.bp[k * 2 + 1];
+#pragma unroll
+      for (int r = 0; r < DIM; r++)
+#pragma unroll
+        for (int c = 0; c < DIM; c++) row[r * stride + bp1 + c] = J[DIM * DIM + r * DIM + c];
+    }
+  }
+  __device__ __forceinline__ void error(const GroupDev<T>& g, int k, int64_t b, T& acc) {
+    T e[DIM];
+    cost<false>(g, k, b, e);
+    const T x = sum_sq<DIM>(e);
+    acc += (g.robust_kind != THB_ROBUST_NONE) ? robust_value(g, k, b, x, DIM) : x;
+  }
+};
+
+template <typename T> struct ReprojectionCost {
+  static constexpr int DIM = 2, NV = 0, NJ = 18;
+  static constexpr bool ROBUST = true;
+  T w[2], J[NJ];   // camera block 2 x 6, then point block 2 x 3
+
+  __device__ __forceinline__ bool load(const GroupDev<T>& g, int k, int64_t b) { return load_weight<T, 2>(g, k, b, w); }
+  __device__ __forceinline__ void linearize(const GroupDev<T>& g, int k, int64_t b, T* e, T*) {
+    reprojection_cost<T, true>(g, k, b, w, e, J, J + 12);
+  }
+  static __device__ __forceinline__ T sqnorm(const T* e) { return e[0] * e[0] + e[1] * e[1]; }
+  __device__ __forceinline__ void store(const GroupDev<T>& g, int k, T* row) const {
+    const int stride = g.a_stride[k];
+    const int bp0 = g.bp[k * 2 + 0], bp1 = g.bp[k * 2 + 1];
+#pragma unroll
+    for (int r = 0; r < 2; r++) {
+#pragma unroll
+      for (int c = 0; c < 6; c++) row[r * stride + bp0 + c] = J[r * 6 + c];
+#pragma unroll
+      for (int c = 0; c < 3; c++) row[r * stride + bp1 + c] = J[12 + r * 3 + c];
+    }
+  }
+  __device__ __forceinline__ void error(const GroupDev<T>& g, int k, int64_t b, T& acc) {
+    T e[2];
+    reprojection_cost<T, false>(g, k, b, w, e, nullptr, nullptr);
+    const T x = sqnorm(e);
+    acc += (g.robust_kind != THB_ROBUST_NONE) ? robust_value(g, k, b, x, 2) : x;
+  }
+};
+
+// A Vector cost function has one variable: its row block is the g.dim x g.dim diagonal of the weights (stride = g.dim).
+template <typename T> struct VectorCost {
+  static constexpr int DIM = 0, NV = 0;
+  static constexpr bool ROBUST = false;
+  const T* wp;
+
+  __device__ __forceinline__ bool load(const GroupDev<T>& g, int k, int64_t b) {
+    wp = g.w[k] + (int64_t)g.bstride[k * 4 + 3] * b;
+    return vector_masked(g, wp);
+  }
+  __device__ __forceinline__ T weight(const GroupDev<T>& g, int r) const { return (g.weight_kind == THB_WEIGHT_SCALE) ? wp[0] : wp[r]; }
+  __device__ __forceinline__ void linearize(const GroupDev<T>& g, int k, int64_t, T*, T* row) const {
+    const int stride = g.a_stride[k];
+    const int bp0 = g.bp[k * 2 + 0];
+    for (int r = 0; r < g.dim; r++) {
+      const T w = weight(g, r);
+      for (int c = 0; c < g.dim; c++) row[r * stride + bp0 + c] = (r == c) ? w : T(0);
+    }
+  }
+  // b = -e, row by row (+0 where masked)
+  __device__ __forceinline__ void residual(const GroupDev<T>& g, int k, int64_t b, bool masked, T* brow) const {
+    const T* x = g.x0[k] + (int64_t)g.bstride[k * 4 + 0] * b;
+    const T* tg = g.aux[k] + (int64_t)g.bstride[k * 4 + 2] * b;
+    for (int r = 0; r < g.dim; r++) brow[r] = masked ? T(0) : -((x[r] - tg[r]) * weight(g, r));
+  }
+  // each row's e * e straight into acc (not summed per cost function first)
+  __device__ __forceinline__ void error(const GroupDev<T>& g, int k, int64_t b, T& acc) const {
+    const T* x = g.x0[k] + (int64_t)g.bstride[k * 4 + 0] * b;
+    const T* tg = g.aux[k] + (int64_t)g.bstride[k * 4 + 2] * b;
+    for (int r = 0; r < g.dim; r++) {
+      const T e = (x[r] - tg[r]) * weight(g, r);
+      acc += e * e;
+    }
+  }
+};
+
+// The weight is applied after the cost, to e and to the staged rows; no robust loss.
+template <typename T, int KIND, int D> struct MpCost {
   using M = Mp<KIND, D>;
+  static constexpr int DIM = M::DIM, NV = M::NV;
+  static constexpr bool ROBUST = false;
+  MpWeight<T, M::DIM, D> W;
+
+  __device__ __forceinline__ bool load(const GroupDev<T>& g, int k, int64_t b) { return W.load(g, k, b); }
+  __device__ __forceinline__ void linearize(const GroupDev<T>& g, int k, int64_t b, T* e, T* row) const {
+    const int stride = g.a_stride[k];
+    int bp[M::NVARS];
+#pragma unroll
+    for (int v = 0; v < M::NVARS; v++) bp[v] = g.bp[k * M::BPW + v];
+    mp_cost<T, KIND, D, true>(g, k, b, e, row, stride, bp);
+    W.apply(e, 1, 1);
+    W.apply(row, stride, stride);
+  }
+  __device__ __forceinline__ void error(const GroupDev<T>& g, int k, int64_t b, T& acc) const {
+    T e[DIM];
+    mp_cost<T, KIND, D, false>(g, k, b, e, nullptr, 0, nullptr);
+    W.apply(e, 1, 1);
+    acc += sum_sq<DIM>(e);
+  }
+};
+
+template <typename T, class Cost>
+__global__ void __launch_bounds__(128) linearize_kernel(GroupDev<T> g, int64_t B, T* __restrict__ A_val, int64_t nnz,
+                                                        T* __restrict__ bvec, int64_t m) {
+  constexpr bool STAGED = Cost::NV > 0;
   extern __shared__ double lin_stage_raw[];
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const bool valid = t < (int64_t)g.K * B;     // (no early exit: every lane takes part in the warp-cooperative store below)
+  const bool valid = t < (int64_t)g.K * B;
+  if (!STAGED && !valid) return;               // (staged: no early exit, every lane takes part in the warp-cooperative store below)
   const int k = valid ? (int)(t / B) : 0;
   const int64_t b = valid ? t - (int64_t)k * B : 0;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  T* stage = reinterpret_cast<T*>(lin_stage_raw) + (size_t)warp * 32 * (M::NV + 1);
-  T* mine = stage + lane * (M::NV + 1);
-  const int stride = g.a_stride[k];
-  const int nv = M::DIM * stride;              // <= NV: the row block spans the cost function's own variables
-  int bp[M::NVARS];
+  T* stage = reinterpret_cast<T*>(lin_stage_raw) + (size_t)warp * 32 * (Cost::NV + 1);
+  auto row = [&]() { return STAGED ? stage + lane * (Cost::NV + 1) : A_val + b * nnz + g.a_off[k]; };
+  Cost c;
+  T e[Cost::DIM > 0 ? Cost::DIM : 1];
+  const bool masked = c.load(g, k, b);
+  if (masked) {
 #pragma unroll
-  for (int v = 0; v < M::NVARS; v++) bp[v] = g.bp[k * M::BPW + v];
-  T e[M::DIM];
-  MpWeight<T, M::DIM, D> W;
-  if (W.load(g, k, b)) {   // every weight of this (k, b) is zero: masked cost function
-#pragma unroll
-    for (int r = 0; r < M::DIM; r++) e[r] = T(0);
-    for (int i = 0; i < nv; i++) mine[i] = T(0);
+    for (int r = 0; r < Cost::DIM; r++) e[r] = T(0);
+    const int nv = (Cost::DIM > 0 ? Cost::DIM : g.dim) * g.a_stride[k];
+    T* z = row();
+    for (int i = 0; i < nv; i++) z[i] = T(0);
   } else {
-    mp_cost<T, KIND, D, true>(g, k, b, e, mine, stride, bp);
-    W.apply(e, 1, 1);
-    W.apply(mine, stride, stride);
+    c.linearize(g, k, b, e, row());
+    if constexpr (Cost::ROBUST) {
+      if (g.robust_kind != THB_ROBUST_NONE) {
+        const T sc = robust_rescale(g, k, b, Cost::sqnorm(e));
+#pragma unroll
+        for (int r = 0; r < Cost::DIM; r++) e[r] *= sc;
+#pragma unroll
+        for (int i = 0; i < Cost::NJ; i++) c.J[i] *= sc;
+      }
+      c.store(g, k, row());
+    }
   }
-  __syncwarp();
-  const unsigned long long my_dst = valid ? reinterpret_cast<unsigned long long>(A_val + b * nnz + g.a_off[k]) : 0ull;
-  for (int i = 0; i < 32; i++) {
-    const unsigned long long d = __shfl_sync(0xffffffffu, my_dst, i);
-    const int nvi = __shfl_sync(0xffffffffu, nv, i);
-    if (d != 0ull) {
-      T* dst = reinterpret_cast<T*>(d);
-      const T* src = stage + i * (M::NV + 1);
-      for (int v = lane; v < nvi; v += 32) dst[v] = src[v];
+  if constexpr (STAGED) {
+    // A cost function's rows of A_val are ONE contiguous run of DIM * stride values per batch item (stride = its row length), but
+    // the items of a warp lie nnz values apart: storing from the computing thread writes 8 bytes to 32 different sectors per
+    // instruction.  The warp's 32 runs are staged in shared memory and the whole warp stores each run with consecutive lanes
+    // (256-byte segments).
+    const int nv = Cost::DIM * g.a_stride[k];   // <= NV: the row block spans the cost function's own variables
+    __syncwarp();
+    const unsigned long long my_dst = valid ? reinterpret_cast<unsigned long long>(A_val + b * nnz + g.a_off[k]) : 0ull;
+    for (int i = 0; i < 32; i++) {
+      const unsigned long long d = __shfl_sync(0xffffffffu, my_dst, i);
+      const int nvi = __shfl_sync(0xffffffffu, nv, i);
+      if (d != 0ull) {
+        T* dst = reinterpret_cast<T*>(d);
+        const T* src = stage + i * (Cost::NV + 1);
+        for (int v = lane; v < nvi; v += 32) dst[v] = src[v];
+      }
     }
   }
   if (valid) {
     T* brow = bvec + b * m + g.row0[k];
+    if constexpr (Cost::DIM > 0) {
 #pragma unroll
-    for (int r = 0; r < M::DIM; r++) brow[r] = -e[r];
+      for (int r = 0; r < Cost::DIM; r++) brow[r] = -e[r];
+    } else {
+      c.residual(g, k, b, masked, brow);
+    }
   }
 }
 
-template <typename T, int KIND, int D>
-__global__ void __launch_bounds__(128) error_mp_kernel(GroupDev<T> g, int64_t B, T* __restrict__ partial) {
-  using M = Mp<KIND, D>;
+// One thread = kErrCostsPerThread cost functions of one batch item; partial[chunk, b] = half their summed squared error.
+template <typename T, class Cost>
+__global__ void __launch_bounds__(128) error_kernel(GroupDev<T> g, int64_t B, T* __restrict__ partial) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int nchunks = (g.K + kErrCostsPerThread - 1) / kErrCostsPerThread;
   if (t >= (int64_t)nchunks * B) return;
@@ -907,15 +863,9 @@ __global__ void __launch_bounds__(128) error_mp_kernel(GroupDev<T> g, int64_t B,
   T acc = T(0);
   const int k1 = min(g.K, (c + 1) * kErrCostsPerThread);
   for (int k = c * kErrCostsPerThread; k < k1; k++) {
-    MpWeight<T, M::DIM, D> W;
-    if (W.load(g, k, b)) continue;
-    T e[M::DIM];
-    mp_cost<T, KIND, D, false>(g, k, b, e, nullptr, 0, nullptr);
-    W.apply(e, 1, 1);
-    T x = T(0);
-#pragma unroll
-    for (int r = 0; r < M::DIM; r++) x += e[r] * e[r];
-    acc += x;
+    Cost cost;
+    if (cost.load(g, k, b)) continue;
+    cost.error(g, k, b, acc);
   }
   partial[(int64_t)c * B + b] = acc * T(0.5);
 }
@@ -1178,142 +1128,80 @@ template <typename T> __global__ void k_se3_compose(const T* __restrict__ G0, co
 // ------------------------------------------------------------------------------------------------
 static inline unsigned grid_for(int64_t total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
+// The motion-planning kinds whose pose dof D varies: the MpCost instance of the dof mp_dof() checked.
+template <typename T, int KIND, class F> static int with_mp_dof(int dof, F& f) {
+  if (dof == 1) return f(MpCost<T, KIND, 1>());
+  if (dof == 2) return f(MpCost<T, KIND, 2>());
+  if (dof == 3) return f(MpCost<T, KIND, 3>());
+  return THB_ERR_BAD_ARG;
+}
+
+// Calls f(Cost()) with the policy of g->kind (and, for the motion-planning kinds, its pose dof) and returns what f returns;
+// THB_ERR_BAD_ARG if the group lacks a field its kind reads, THB_ERR_UNSUPPORTED for an unknown kind.
+template <typename T, class F> static int with_cost_kind(const thb_cost_group* g, F f) {
+  const int dof = mp_dof(g);   // 0 for the other kinds
+  switch (g->kind) {
+    case THB_COST_BETWEEN_SE3: return f(LieCost<T, THB_COST_BETWEEN_SE3>());
+    case THB_COST_LOCAL_SE3: return f(LieCost<T, THB_COST_LOCAL_SE3>());
+    case THB_COST_BETWEEN_SO3: return f(LieCost<T, THB_COST_BETWEEN_SO3>());
+    case THB_COST_LOCAL_SO3: return f(LieCost<T, THB_COST_LOCAL_SO3>());
+    case THB_COST_BETWEEN_SE2: return f(LieCost<T, THB_COST_BETWEEN_SE2>());
+    case THB_COST_LOCAL_SE2: return f(LieCost<T, THB_COST_LOCAL_SE2>());
+    case THB_COST_LOCAL_VECTOR: return f(VectorCost<T>());
+    case THB_COST_REPROJECTION:
+      if (g->aux2 == nullptr || g->aux3 == nullptr || g->aux4 == nullptr || g->bstride2 == nullptr) return THB_ERR_BAD_ARG;
+      return f(ReprojectionCost<T>());
+    case THB_COST_COLLISION2D_POINT2: return dof ? f(MpCost<T, THB_COST_COLLISION2D_POINT2, 2>()) : THB_ERR_BAD_ARG;
+    case THB_COST_COLLISION2D_SE2: return dof ? f(MpCost<T, THB_COST_COLLISION2D_SE2, 3>()) : THB_ERR_BAD_ARG;
+    case THB_COST_DOUBLE_INTEGRATOR_SE2: return dof ? f(MpCost<T, THB_COST_DOUBLE_INTEGRATOR_SE2, 3>()) : THB_ERR_BAD_ARG;
+    case THB_COST_NONHOLONOMIC_SE2: return dof ? f(MpCost<T, THB_COST_NONHOLONOMIC_SE2, 3>()) : THB_ERR_BAD_ARG;
+    case THB_COST_NONHOLONOMIC_VECTOR: return dof ? f(MpCost<T, THB_COST_NONHOLONOMIC_VECTOR, 3>()) : THB_ERR_BAD_ARG;
+    case THB_COST_QUASI_STATIC_PUSHING_PLANAR: return dof ? f(MpCost<T, THB_COST_QUASI_STATIC_PUSHING_PLANAR, 3>()) : THB_ERR_BAD_ARG;
+    case THB_COST_EFF_OBJ_CONTACT_PLANAR: return dof ? f(MpCost<T, THB_COST_EFF_OBJ_CONTACT_PLANAR, 3>()) : THB_ERR_BAD_ARG;
+    case THB_COST_DOUBLE_INTEGRATOR_VECTOR: return with_mp_dof<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR>(dof, f);
+    case THB_COST_HINGE: return with_mp_dof<T, THB_COST_HINGE>(dof, f);
+    default: return THB_ERR_UNSUPPORTED;
+  }
+}
+
+// A kernel instance that needs more than the default 48 KB of dynamic shared memory opts in, once.
+template <typename T, class Cost> static int allow_linearize_smem(size_t smem) {
+  static bool done = false;
+  if (!done && smem > 48 * 1024) {
+    THB_CUDA(cudaFuncSetAttribute(linearize_kernel<T, Cost>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    done = true;
+  }
+  return THB_OK;
+}
+
 template <typename T>
 static int linearize_group(const thb_cost_group* g, int64_t B, T* A_val, int64_t nnz, T* b, int64_t m, thb_stream_t s) {
   if (g == nullptr || g->K < 0 || B < 0) return THB_ERR_BAD_ARG;
   if (g->K == 0 || B == 0) return THB_OK;
-  GroupDev<T> d = to_dev<T>(g);
-  const int64_t total = (int64_t)g->K * B;
-  const unsigned grid = grid_for(total, 128);
-  cudaStream_t cs = thb_cs(s);
-#define THB_LIN_LAUNCH(KIND, NV)                                                                                              \
-  do {                                                                                                                      \
-    const size_t smem_ = (size_t)4 * 32 * ((NV) + 1) * sizeof(T);                                                           \
-    static bool attr_ = false;                                                                                              \
-    if (!attr_ && smem_ > 48 * 1024) {                                                                                      \
-      THB_CUDA(cudaFuncSetAttribute(linearize_kernel<T, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_));   \
-      attr_ = true;                                                                                                         \
-    }                                                                                                                       \
-    linearize_kernel<T, KIND><<<grid, 128, smem_, cs>>>(d, B, A_val, nnz, b, m);                                            \
-  } while (0)
-  switch (g->kind) {
-    case THB_COST_BETWEEN_SE3: THB_LIN_LAUNCH(THB_COST_BETWEEN_SE3, 72); break;
-    case THB_COST_LOCAL_SE3: THB_LIN_LAUNCH(THB_COST_LOCAL_SE3, 36); break;
-    case THB_COST_BETWEEN_SO3: THB_LIN_LAUNCH(THB_COST_BETWEEN_SO3, 18); break;
-    case THB_COST_LOCAL_SO3: THB_LIN_LAUNCH(THB_COST_LOCAL_SO3, 9); break;
-    case THB_COST_BETWEEN_SE2: THB_LIN_LAUNCH(THB_COST_BETWEEN_SE2, 18); break;
-    case THB_COST_LOCAL_SE2: THB_LIN_LAUNCH(THB_COST_LOCAL_SE2, 9); break;
-    case THB_COST_LOCAL_VECTOR: linearize_vector_kernel<T><<<grid, 128, 0, cs>>>(d, B, A_val, nnz, b, m); break;
-    case THB_COST_REPROJECTION:
-      if (g->aux2 == nullptr || g->aux3 == nullptr || g->aux4 == nullptr || g->bstride2 == nullptr) return THB_ERR_BAD_ARG;
-      linearize_reprojection_kernel<T><<<grid, 128, 0, cs>>>(d, B, A_val, nnz, b, m);
-      break;
-    case THB_COST_COLLISION2D_POINT2:
-    case THB_COST_COLLISION2D_SE2:
-    case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
-    case THB_COST_DOUBLE_INTEGRATOR_SE2:
-    case THB_COST_HINGE:
-    case THB_COST_NONHOLONOMIC_SE2:
-    case THB_COST_NONHOLONOMIC_VECTOR:
-    case THB_COST_QUASI_STATIC_PUSHING_PLANAR:
-    case THB_COST_EFF_OBJ_CONTACT_PLANAR: {
-      const int dof = mp_dof(g);
-      if (dof == 0) return THB_ERR_BAD_ARG;
-#define THB_MP_LAUNCH(KIND, D)                                                                                                \
-  do {                                                                                                                      \
-    const size_t smem_ = (size_t)4 * 32 * (Mp<KIND, D>::NV + 1) * sizeof(T);                                                \
-    static bool attr_ = false;                                                                                              \
-    if (!attr_ && smem_ > 48 * 1024) {                                                                                      \
-      THB_CUDA(cudaFuncSetAttribute(linearize_mp_kernel<T, KIND, D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_)); \
-      attr_ = true;                                                                                                         \
-    }                                                                                                                       \
-    linearize_mp_kernel<T, KIND, D><<<grid, 128, smem_, cs>>>(d, B, A_val, nnz, b, m);                                      \
-  } while (0)
-      switch (g->kind) {
-        case THB_COST_COLLISION2D_POINT2: THB_MP_LAUNCH(THB_COST_COLLISION2D_POINT2, 2); break;
-        case THB_COST_COLLISION2D_SE2: THB_MP_LAUNCH(THB_COST_COLLISION2D_SE2, 3); break;
-        case THB_COST_DOUBLE_INTEGRATOR_SE2: THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_SE2, 3); break;
-        case THB_COST_NONHOLONOMIC_SE2: THB_MP_LAUNCH(THB_COST_NONHOLONOMIC_SE2, 3); break;
-        case THB_COST_NONHOLONOMIC_VECTOR: THB_MP_LAUNCH(THB_COST_NONHOLONOMIC_VECTOR, 3); break;
-        case THB_COST_QUASI_STATIC_PUSHING_PLANAR: THB_MP_LAUNCH(THB_COST_QUASI_STATIC_PUSHING_PLANAR, 3); break;
-        case THB_COST_EFF_OBJ_CONTACT_PLANAR: THB_MP_LAUNCH(THB_COST_EFF_OBJ_CONTACT_PLANAR, 3); break;
-        case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
-          if (dof == 1) THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 1);
-          else if (dof == 2) THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 2);
-          else THB_MP_LAUNCH(THB_COST_DOUBLE_INTEGRATOR_VECTOR, 3);
-          break;
-        default:   // THB_COST_HINGE
-          if (dof == 1) THB_MP_LAUNCH(THB_COST_HINGE, 1);
-          else if (dof == 2) THB_MP_LAUNCH(THB_COST_HINGE, 2);
-          else THB_MP_LAUNCH(THB_COST_HINGE, 3);
-          break;
-      }
-#undef THB_MP_LAUNCH
-      break;
-    }
-    default: return THB_ERR_UNSUPPORTED;
-  }
-  THB_CHECK_LAUNCH();
-  return THB_OK;
+  const GroupDev<T> d = to_dev<T>(g);
+  const unsigned grid = grid_for((int64_t)g->K * B, 128);
+  return with_cost_kind<T>(g, [&](auto cost) {
+    using Cost = decltype(cost);
+    const size_t smem = Cost::NV > 0 ? (size_t)4 * 32 * (Cost::NV + 1) * sizeof(T) : 0;   // 4 warps x 32 staged rows
+    const int rc = allow_linearize_smem<T, Cost>(smem);
+    if (rc != THB_OK) return rc;
+    linearize_kernel<T, Cost><<<grid, 128, smem, thb_cs(s)>>>(d, B, A_val, nnz, b, m);
+    THB_CHECK_LAUNCH();
+    return THB_OK;
+  });
 }
 
 template <typename T> static int error_group(const thb_cost_group* g, int64_t B, T* partial, thb_stream_t s) {
   if (g == nullptr || g->K < 0 || B < 0) return THB_ERR_BAD_ARG;
   if (g->K == 0 || B == 0) return THB_OK;
-  GroupDev<T> d = to_dev<T>(g);
+  const GroupDev<T> d = to_dev<T>(g);
   const int nchunks = (g->K + kErrCostsPerThread - 1) / kErrCostsPerThread;
   const unsigned grid = grid_for((int64_t)nchunks * B, 128);
-  cudaStream_t cs = thb_cs(s);
-  switch (g->kind) {
-    case THB_COST_BETWEEN_SE3: error_kernel<T, THB_COST_BETWEEN_SE3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-    case THB_COST_LOCAL_SE3: error_kernel<T, THB_COST_LOCAL_SE3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-    case THB_COST_BETWEEN_SO3: error_kernel<T, THB_COST_BETWEEN_SO3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-    case THB_COST_LOCAL_SO3: error_kernel<T, THB_COST_LOCAL_SO3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-    case THB_COST_BETWEEN_SE2: error_kernel<T, THB_COST_BETWEEN_SE2><<<grid, 128, 0, cs>>>(d, B, partial); break;
-    case THB_COST_LOCAL_SE2: error_kernel<T, THB_COST_LOCAL_SE2><<<grid, 128, 0, cs>>>(d, B, partial); break;
-    case THB_COST_LOCAL_VECTOR: error_vector_kernel<T><<<grid, 128, 0, cs>>>(d, B, partial); break;
-    case THB_COST_REPROJECTION:
-      if (g->aux2 == nullptr || g->aux3 == nullptr || g->aux4 == nullptr || g->bstride2 == nullptr) return THB_ERR_BAD_ARG;
-      error_reprojection_kernel<T><<<grid, 128, 0, cs>>>(d, B, partial);
-      break;
-    case THB_COST_COLLISION2D_POINT2:
-    case THB_COST_COLLISION2D_SE2:
-    case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
-    case THB_COST_DOUBLE_INTEGRATOR_SE2:
-    case THB_COST_HINGE:
-    case THB_COST_NONHOLONOMIC_SE2:
-    case THB_COST_NONHOLONOMIC_VECTOR:
-    case THB_COST_QUASI_STATIC_PUSHING_PLANAR:
-    case THB_COST_EFF_OBJ_CONTACT_PLANAR: {
-      const int dof = mp_dof(g);
-      if (dof == 0) return THB_ERR_BAD_ARG;
-      switch (g->kind) {
-        case THB_COST_COLLISION2D_POINT2: error_mp_kernel<T, THB_COST_COLLISION2D_POINT2, 2><<<grid, 128, 0, cs>>>(d, B, partial); break;
-        case THB_COST_COLLISION2D_SE2: error_mp_kernel<T, THB_COST_COLLISION2D_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-        case THB_COST_DOUBLE_INTEGRATOR_SE2: error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-        case THB_COST_NONHOLONOMIC_SE2: error_mp_kernel<T, THB_COST_NONHOLONOMIC_SE2, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-        case THB_COST_NONHOLONOMIC_VECTOR: error_mp_kernel<T, THB_COST_NONHOLONOMIC_VECTOR, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-        case THB_COST_QUASI_STATIC_PUSHING_PLANAR:
-          error_mp_kernel<T, THB_COST_QUASI_STATIC_PUSHING_PLANAR, 3><<<grid, 128, 0, cs>>>(d, B, partial);
-          break;
-        case THB_COST_EFF_OBJ_CONTACT_PLANAR: error_mp_kernel<T, THB_COST_EFF_OBJ_CONTACT_PLANAR, 3><<<grid, 128, 0, cs>>>(d, B, partial); break;
-        case THB_COST_DOUBLE_INTEGRATOR_VECTOR:
-          if (dof == 1) error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 1><<<grid, 128, 0, cs>>>(d, B, partial);
-          else if (dof == 2) error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 2><<<grid, 128, 0, cs>>>(d, B, partial);
-          else error_mp_kernel<T, THB_COST_DOUBLE_INTEGRATOR_VECTOR, 3><<<grid, 128, 0, cs>>>(d, B, partial);
-          break;
-        default:   // THB_COST_HINGE
-          if (dof == 1) error_mp_kernel<T, THB_COST_HINGE, 1><<<grid, 128, 0, cs>>>(d, B, partial);
-          else if (dof == 2) error_mp_kernel<T, THB_COST_HINGE, 2><<<grid, 128, 0, cs>>>(d, B, partial);
-          else error_mp_kernel<T, THB_COST_HINGE, 3><<<grid, 128, 0, cs>>>(d, B, partial);
-          break;
-      }
-      break;
-    }
-    default: return THB_ERR_UNSUPPORTED;
-  }
-  THB_CHECK_LAUNCH();
-  return THB_OK;
+  return with_cost_kind<T>(g, [&](auto cost) {
+    error_kernel<T, decltype(cost)><<<grid, 128, 0, thb_cs(s)>>>(d, B, partial);
+    THB_CHECK_LAUNCH();
+    return THB_OK;
+  });
 }
 
 template <typename T>
